@@ -6,8 +6,8 @@
 
 One JSON line on stdout (rank 0).  A "step" is one Allreduce of S bytes per rank (default
 S = 256 MiB, the headline point) on synthetic uniform[0,1) buffers; out of place, so the input
-is identical every step.  Send+recv buffers (2 x 256 MiB) exceed the 126 MB L2, so no flush is
-needed between steps.
+is identical every step.  Send+recv buffers (2 x 256 MiB) exceed the 50 MB L2 of an H100, so no
+flush is needed between steps.
 
   value     N >= 2: bus bandwidth, nccl-tests convention: S/t * 2(N-1)/N, GB = 1e9 B, device
             resident buffers, t = CUDA-event time over K back-to-back steps / K, max over ranks.
@@ -29,14 +29,18 @@ needed between steps.
             on the same buffers (comparison line only, run last and under a deadline; NCCL is never
             on the product path).  roofline.nvlink_counters: hardware link byte counts
             (nvidia-smi nvlink) around 50 more steps of the timed call, when the tool exposes them.
-  roofline  N == 1: HBM (read S + write S per launch) against MEASURED_PEAKS.json hbm_gbs;
-            N >= 2: NVLink, busbw against 900 GB/s nominal (measured peer copy ~770 GB/s) plus the
-            HBM side ((3 - 1/N) * S per launch).
+  roofline  N == 1: HBM (read S + write S per launch) against the H100 SXM data sheet's 3.35 TB/s;
+            N >= 2: NVLink, busbw against 450 GB/s per direction (H100 SXM, NVLink 4, nominal) plus
+            the HBM side ((3 - 1/N) * S per launch).
   cpu_baseline / --impl reference: oracle/ref_tcp.c, the restated gob-over-TCP-loopback path of
             the reference (it has no Allreduce; composed as a ring over Send/Receive), SAME
             config: S bytes per rank, N ranks, same steps/warm-up unless that exceeds ~90 s (then
             capped, and config.steps_capped says so).  The only uses of oracle/ here are that
             baseline, the input generator and the parity checks -- never the measured path.
+  --dump-outputs DIR   after the timed steps, rank 0 writes what the last one returned (the recv
+            buffer) as DIR/allreduce_recv.npy, float32: whole up to DUMP_MAX_ELEMS elements, else a
+            fixed seeded sample of that many.  Inputs depend on the arguments only, so two builds
+            run with the same arguments can be compared output for output.
 """
 import argparse
 import ctypes
@@ -53,10 +57,10 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 
 SEED = 0xB2000000
-NVLINK_NOMINAL_GBS = 900.0   # per direction per GPU (B200_PROFILING.md)
-NVLINK_MEASURED_GBS = 770.0  # peer copy measured on this pool (B200_PROFILING.md)
-HBM_FALLBACK_GBS = 6650.0
+NVLINK_NOMINAL_GBS = 450.0   # per direction per GPU: H100 SXM, 18 NVLink 4 links (data sheet: 900 GB/s both ways)
+HBM_PEAK_GBS = 3350.0        # H100 SXM HBM3, data sheet
 BLOCK = 1 << 22              # elements per parity block
+DUMP_MAX_ELEMS = 8 << 20     # --dump-outputs: 32 MiB of float32 at most
 
 
 def world_from_env(args):
@@ -73,7 +77,7 @@ def world_from_env(args):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, gpu):
         super().__init__(daemon=True)
@@ -114,24 +118,20 @@ class ClockSampler(threading.Thread):
         return {"sm_mhz": (load[len(load) // 2] if load else None), "sm_max_mhz": mx or None, "reasons": sorted(reasons), "samples": len(sm)}
 
 
-def measured_peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return json.load(f), "measured"
-    except Exception:  # noqa: BLE001
-        return {"hbm_gbs": HBM_FALLBACK_GBS}, "fallback"
-
-
-def measured_traffic(n, nbytes, kernel):
-    """dram read+write bytes per launch from the committed ncu captures (profiles/traffic.json)."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            for e in json.load(f)["entries"]:
-                if e["n"] == n and e["bytes"] == nbytes and e["kernel"] == kernel:
-                    return e["traffic_bytes"], e["source"]
-    except Exception:  # noqa: BLE001
-        pass
-    return None, None
+def dump_outputs(out_dir, recv, count):
+    """recv (float32, `count` elements) as out_dir/allreduce_recv.npy: whole when it holds at most
+    DUMP_MAX_ELEMS elements, else one element drawn at a seeded offset from each of DUMP_MAX_ELEMS
+    equal strata, so the sample covers the whole buffer and is the same in every run."""
+    os.makedirs(out_dir, exist_ok=True)
+    host = np.empty(count, dtype=np.float32)
+    for lo in range(0, count, BLOCK):
+        m = min(BLOCK, count - lo)
+        host[lo:lo + m] = recv[lo:lo + m].to_host()
+    if count > DUMP_MAX_ELEMS:
+        stride = count // DUMP_MAX_ELEMS
+        offs = np.random.default_rng(SEED).integers(0, stride, DUMP_MAX_ELEMS)
+        host = host[np.arange(DUMP_MAX_ELEMS, dtype=np.int64) * stride + offs]
+    np.save(os.path.join(out_dir, "allreduce_recv.npy"), host)
 
 
 def nvlink_counters(gpu):
@@ -303,7 +303,10 @@ def main():
     ap.add_argument("--no-nccl", action="store_true")
     ap.add_argument("--deadline", type=int, default=300, help="seconds after which a partial contract line is printed and the run ends")
     ap.add_argument("--nccl-deadline", type=int, default=60, help="seconds the NCCL comparison may take before it is abandoned")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's result under DIR (see the module doc)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.warmup < 3:
         args.warmup = 3
     rank, world, local, addr, addrs = world_from_env(args)
@@ -585,6 +588,10 @@ def main():
     launches = int(lib.b200mpi_launch_count() - l0)
     mpi.Barrier()
     t_step = max_over_ranks(ms.value / 1e3 / args.steps)
+    if args.dump_outputs:
+        if rank == 0:
+            dump_outputs(args.dump_outputs, recv, count)
+        mpi.Barrier()
 
     algbw = S / t_step / 1e9
     value = algbw * bus
@@ -597,8 +604,8 @@ def main():
                        "note": "partial line: a later section of bench.py did not finish before --deadline"},
             "algbw_gbs": algbw, "e2e": None, "gpu_launches": launches, "clocks": None,
             "roofline": {"bound": "hbm" if n == 1 else "nvlink", "achieved": (2 * S / t_step / 1e9) if n == 1 else value,
-                         "peak": HBM_FALLBACK_GBS if n == 1 else NVLINK_NOMINAL_GBS, "unit": "GB/s",
-                         "frac": ((2 * S / t_step / 1e9) / HBM_FALLBACK_GBS) if n == 1 else value / NVLINK_NOMINAL_GBS, "traffic": None},
+                         "peak": HBM_PEAK_GBS if n == 1 else NVLINK_NOMINAL_GBS, "unit": "GB/s",
+                         "frac": ((2 * S / t_step / 1e9) / HBM_PEAK_GBS) if n == 1 else value / NVLINK_NOMINAL_GBS, "traffic": None},
             "parity": dict(parity), "parity_ok": parity_ok}
 
     def deadline_bail():
@@ -789,8 +796,7 @@ def main():
         raise RuntimeError(L.last_error())
     clocks = sampler.stop()
     clocks["window"] = "timed region + e2e region + secondary + 0.6 s of the same launches (sampler period 100 ms)"
-    peaks, peak_kind = measured_peaks()
-    hbm_peak = float(peaks.get("hbm_gbs", HBM_FALLBACK_GBS))
+    hbm_peak, peak_kind = HBM_PEAK_GBS, "H100 SXM data sheet (nominal)"
     if n == 1:
         roof = {"bound": "hbm", "achieved": 2 * S / t_step / 1e9, "peak": hbm_peak, "unit": "GB/s",
                 "frac": 2 * S / t_step / 1e9 / hbm_peak, "traffic": None, "peak_source": peak_kind,
@@ -799,8 +805,8 @@ def main():
         hbm_bytes = (3.0 - 1.0 / n) * S
         aname = L.ALGO_NAMES.get(algo_used, "?")
         roof = {"bound": "nvlink", "achieved": value, "peak": NVLINK_NOMINAL_GBS, "unit": "GB/s",
-                "frac": value / NVLINK_NOMINAL_GBS, "frac_of_measured_peer_copy": value / NVLINK_MEASURED_GBS,
-                "traffic": None, "peak_source": "nominal NVLink 5 per direction per GPU; measured peer copy %.0f GB/s" % NVLINK_MEASURED_GBS,
+                "frac": value / NVLINK_NOMINAL_GBS,
+                "traffic": None, "peak_source": "H100 SXM data sheet: NVLink 4, nominal, per direction per GPU",
                 "kernel": "allreduce_%s_kernel" % aname,
                 "nvls_link_bytes_per_launch": (1.0 + 1.0 / n) * S if aname == "nvls" else None,
                 "algorithmic_bytes_per_launch": 2.0 * (n - 1) / n * S,
@@ -808,10 +814,6 @@ def main():
 
     if n > 1:
         roof["nvlink_counters"] = nvl
-    traffic, tsrc = measured_traffic(n, S, roof["kernel"])
-    if traffic is not None:
-        roof["traffic"] = traffic
-        roof["traffic_source"] = tsrc
 
     cpu = None
     if rank == 0 and n == 1 and not args.no_cpu_baseline:

@@ -1,4 +1,4 @@
-// Package mpi is the drop-in facade for github.com/btracey/mpi on a box of NVIDIA B200 GPUs.
+// Package mpi is the drop-in facade for github.com/btracey/mpi on a box of NVIDIA H100 GPUs.
 //
 // UNVERIFIED: this image has no Go toolchain, so these files have never been compiled.  They are
 // the binding a maintainer adds; the C ABI they call (include/b200mpi.h) is exercised end to end

@@ -1,5 +1,5 @@
 /*
- * b200mpi.h -- C ABI of libb200mpi.so: the B200-native transport that sits behind the
+ * b200mpi.h -- C ABI of libb200mpi.so: the H100-native transport that sits behind the
  * btracey/mpi Go facade (mpi.Init/Finalize/Rank/Size/Send/Receive + the new
  * Recv/Bcast/Allreduce/Allgather entry points).
  *

@@ -1,4 +1,4 @@
-"""mpi_b200 -- B200-native transport behind the btracey/mpi API.
+"""mpi_b200 -- H100-native transport behind the btracey/mpi API.
 
 `import mpi_b200 as mpi` gives the reference's package surface (mpi.go) over libb200mpi.so:
 Init, Finalize, Rank, Size, Send, Receive (+ Recv, Bcast, Allreduce, Allgather, Barrier,

@@ -155,7 +155,7 @@ class Interface(abc.ABC):
 
 
 class Cuda(Interface):
-    """The B200 implementation behind the facade; plays the role of `Network`
+    """The H100 implementation behind the facade; plays the role of `Network`
     (network.go:25-39): public fields win over flags (network.go:69-90)."""
 
     def __init__(self, Addr="", Addrs=None, Timeout=0, Password="", Gpu=None):

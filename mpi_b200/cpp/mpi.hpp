@@ -179,7 +179,7 @@ struct Interface {
   virtual Error Wait(int, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Wait"; return e; }
 };
 
-// The B200 implementation; plays the role of `Network` (network.go:25-39): fields win over flags.
+// The H100 implementation; plays the role of `Network` (network.go:25-39): fields win over flags.
 struct Cuda : Interface {
   std::string Addr;
   std::vector<std::string> Addrs;

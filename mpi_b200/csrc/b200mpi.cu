@@ -5,7 +5,7 @@
 //   Network.Send / Receive (+tagManager)    network.go:449-625         -> b200mpi_send / _recv
 //   local (same-rank rendezvous)            network.go:388-446         -> same mailbox, own pair
 //   AllReduce stub                          mpi.go:130                 -> b200mpi_allreduce, _bcast, _allgather
-// The data never touches a socket: payloads move by sm_100a kernels (kernels.cuh) through the
+// The data never touches a socket: payloads move by sm_90a kernels (kernels.cuh) through the
 // peer-mapped heaps (heap.h).  There is no CPU implementation of any data call: without a CUDA
 // device every one of them fails with B200MPI_ERR_NO_DEVICE.
 #include <cuda.h>
@@ -147,14 +147,14 @@ struct Ctx {
   int bcast_nvls2 = 1;         // Bcast NVLS: scatter + multicast (1) or root-only multicast (0)
   size_t bcast_nvls_min = 0, allgather_nvls_min = 0; // AUTO thresholds (bytes), set at init from n
   int twoshot_unroll = 1; // 0: 1/2/4 vectors per thread for n = 8/4/2, 1: 2/4/8
-  int nvls_unroll = 2;      // 8 GPUs, 256 MiB: unroll 2 x 64 CTAs 810 GB/s, 4 x 148 CTAs 780 (profiles/r01/sweep_n8_nvls_blocks_unroll_v2.jsonl)
-  int nvls_max_blocks = 48; // fewer requests in flight suit the switch reduction better (r02: 48 CTAs 822/845 GB/s at 256 MiB/1 GiB, 64 CTAs 817/840)
+  int nvls_unroll = 2;      // multi-GPU switch tuning: not yet measured on H100 (tools/sweep.py re-derives it)
+  int nvls_max_blocks = 48; // fewer requests in flight suit the switch reduction; not yet measured on H100
   size_t ll_max_bytes = 0; // AUTO uses the barrier-free LL allreduce for messages up to this size (<= 256 KiB)
   uint32_t ll_seq = 0;
   // pinned, device-mapped bounce buffers: a small host-slice Allreduce is a memcpy + ONE kernel that
   // reads its input over PCIe and writes result + completion word to host memory
   char* ll_host = nullptr; char* ll_dev = nullptr; // [in kLLCells*8][out kLLCells*8][done word]
-  int copy_variant = 5; // 16 vectors in flight per thread, 256 threads: best of 8 launch shapes at 256 MiB and 1 GiB
+  int copy_variant = 5; // 16 vectors in flight per thread, 256 threads: best of 7 launch shapes on an H100 SXM (400 W limit), 1.42 TB/s algbw at 256 MiB, 1.43 at 1 GiB
   size_t hybrid_min_bytes = 32u << 20;
   int nvls_min_ranks = 4; // below this the fused two-shot moves fewer bytes per link than NVLS
   size_t own_block_bytes = 1u << 20; // interleave granularity of slice ownership (Owner in kernels.cuh)
@@ -347,7 +347,7 @@ static int launch_copy(void* dst, const void* src, size_t bytes, cudaStream_t s)
     size_t cap = g->max_blocks > 0 ? (size_t)g->max_blocks : (size_t)sms * per_sm;
     return (int)std::max<size_t>(1, std::min(want, cap));
   };
-  switch (g->copy_variant) { // launch shapes for the HBM-bound local copy; see profiles/r01/SUMMARY.md
+  switch (g->copy_variant) { // launch shapes for the HBM-bound local copy (bench.py --params copy_variant=N)
     case 1: copy_bytes_kernel<8, 512, 1><<<grid(512, 8, 1), 512, 0, s>>>(d, c, bytes); break;
     case 2: copy_bytes_kernel<4, 256, 2><<<grid(256, 4, 2), 256, 0, s>>>(d, c, bytes); break;
     case 3: copy_bytes_kernel<8, 256, 2><<<grid(256, 8, 2), 256, 0, s>>>(d, c, bytes); break;
@@ -632,8 +632,8 @@ static int launch_reduce_scatter(int algo, int dtype, int op, uint64_t so, uint6
   return fail(B200MPI_ERR_UNSUPPORTED, "reduce_scatter: dtype must be f32, f64 or i64");
 }
 
-// AUTO for Allreduce.  Thresholds come from the sweeps on 2/4/8 B200s (profiles/r01, profiles/r02):
-// best busbw / latency per (n, size) among the variants.
+// AUTO for Allreduce: best busbw / latency per (n, size) among the variants.  The multi-GPU thresholds
+// have not been measured on H100 yet (tools/sweep.py re-derives them on a box with 2/4/8 GPUs).
 // chunk: the launch is one piece of a pipelined host-slice call, where the barrier-free LL kernel
 // (own sequence numbers, no heap offsets) does not apply.
 static int pick_allreduce(size_t bytes, int dtype, int op, bool chunk = false) {
@@ -661,7 +661,7 @@ static int pick_allreduce(size_t bytes, int dtype, int op, bool chunk = false) {
     return bytes < (2u << 20) ? B200MPI_ALGO_TWOSHOT : big;
   }
   if (bytes <= g->oneshot_max_bytes) return B200MPI_ALGO_ONESHOT;
-  return B200MPI_ALGO_TWOSHOT; // n == 2: LDG and TMA-staged two-shot tie (637 vs 636 GB/s at 256 MiB)
+  return B200MPI_ALGO_TWOSHOT; // n == 2: the LDG and the TMA-staged two-shot move the same bytes per link
 }
 
 // AUTO for Bcast: the switch multicast wins up to a few MiB (one store stream, no second hop); the
@@ -1584,20 +1584,16 @@ int b200mpi_size(void) { return (g && g->initialised) ? g->ctrl.n : 0; }
 int b200mpi_device(void) { return (g && g->initialised && !g->control_only) ? g->dev : -1; }
 int64_t b200mpi_launch_count(void) { return g ? g->launches.load() : 0; }
 
-// Size thresholds of the AUTO policies, from the 2/4/8-GPU sweeps (profiles/r02/SUMMARY.md).
+// Size thresholds of the AUTO policies (multi-GPU; not yet measured on H100).
 // Functions of n (and of whether the switch path exists) only, so every rank agrees.
 static void apply_defaults() {
   const int n = g->ctrl.n;
   const bool nvls = g->heap.mc_base != 0;
   g->ll_max_bytes = 0;
-  // device time, LL vs the best barrier kernel (profiles/r02): 2 GPUs 256 KiB 12.3 us vs 14.5; 4 GPUs 256 KiB 9.5 vs 13.2;
-  // 8 GPUs: see SUMMARY.md section 6
-  // 8 GPUs (two-phase kernel): 1 KiB 6.9 us vs 12.7, 32 KiB 8.6 vs 12.7, 256 KiB 12.9 vs 15.3 -> LL over its whole range
+  // LL (no barrier, one exchange latency) over its whole range on real multi-GPU worlds
   if (!g->shared_device) g->ll_max_bytes = std::min<size_t>(256u << 10, ll_cells(n) * 8);
-  // Measured on 8 B200s (profiles/r02/sweep_n8_bcag_v1.jsonl, sweep_n8_hybrid_v1.jsonl): multicast
-  // delivery tops out near 480-510 GB/s of ingress per GPU, below what plain P2P stores reach
-  // (620-650), so above a few MiB Bcast and Allgather stay on the P2P kernels; mixing P2P traffic
-  // into the NVLS allreduce only slows it (817 -> 793 GB/s at 10 %), so the hybrid stays off.
+  // Above a few MiB Bcast and Allgather stay on the P2P kernels, and the hybrid allreduce stays off,
+  // until multicast delivery has been measured against plain P2P stores on H100.
   g->bcast_nvls_min = SIZE_MAX;
   g->allgather_nvls_min = SIZE_MAX;
   g->hybrid_p2p_permille = 0;
@@ -1653,7 +1649,7 @@ int b200mpi_init(const char* addr, const char* alladdr_csv, const char* password
   cudaDeviceProp prop;
   cudaGetDeviceProperties(&prop, g->dev);
   g->sm_count = prop.multiProcessorCount;
-  if (prop.major < 10) return bail(B200MPI_ERR_NO_DEVICE, std::string("device '") + prop.name + "' is not sm_100-class; this library ships sm_100a code only");
+  if (prop.major != 9 || prop.minor != 0) return bail(B200MPI_ERR_NO_DEVICE, std::string("device '") + prop.name + "' is not sm_90 (H100-class); this library ships sm_90a code only");
   if (!g->drv.load(err)) return bail(B200MPI_ERR_CUDA, err);
   if (!(getenv("B200MPI_NUMA") && atoi(getenv("B200MPI_NUMA")) == 0)) g->gpu_numa_node = numa_node_of_gpu(g->dev);
   if (const char* w = getenv("B200MPI_SCRUB_EVERY")) {

@@ -1,10 +1,10 @@
-// kernels.cuh -- sm_100a device code of libb200mpi: the data plane that replaces the
+// kernels.cuh -- sm_90a (H100) device code of libb200mpi: the data plane that replaces the
 // reference's gob-over-TCP Send/Receive (/root/reference/network.go:518-625) and implements the
 // collectives the reference only stubs (/root/reference/mpi.go:130).
 //
 // Memory model.  Every rank owns one cuMem heap; all heaps are mapped into every rank's address
 // space (Comm::base[r]) so a kernel reaches rank r's memory with plain ld/st.global that the
-// GPU routes over NVLink 5 / NVSwitch (or stays local when r is this rank or shares the device).
+// GPU routes over NVLink 4 / NVSwitch (or stays local when r is this rank or shares the device).
 // The first kCtrlBytes of each heap are control words:
 //     Slot slots[kMaxBlocks][kMaxRanks]   cross-rank flag + per-call buffer descriptor
 //     u32  ring[kMaxBlocks]               ring step counters
@@ -26,7 +26,7 @@
 namespace b200 {
 
 constexpr int kMaxRanks = 8;
-constexpr int kMaxBlocks = 592;            // 148 SMs x 4
+constexpr int kMaxBlocks = 528;            // 132 SMs x 4
 constexpr size_t kCtrlBytes = 16u << 20;   // control region at the start of every heap (== kHeapReserved, heap.h)
 constexpr size_t kRingFlagsOff = 512u << 10;
 constexpr size_t kLLStateOff = 768u << 10;   // LL bookkeeping words (device-resident sequence number, CTA counter)
@@ -934,8 +934,7 @@ allreduce_nvls_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t count
 }
 
 // ---------------------------------------------------------------------------------------------
-// Allreduce, hybrid: the switch reduction (multimem) saturates below the link rate
-// (profiles/r01: 256 MiB..1 GiB x 8 GPUs flat at ~480 GB/s algbw whatever the launch shape), so a
+// Allreduce, hybrid: for when the switch reduction (multimem) saturates below the link rate, so a
 // part of the message goes the P2P way at the same time: CTAs [0, nb_nvls) run nvls_body on
 // vectors [0, split), the remaining CTAs run the fused P2P two-shot body on [split, nvec) and the
 // tail.  Every element is still reduced exactly once by its owner and the same bits reach every
@@ -1451,10 +1450,9 @@ copy_bytes_kernel(unsigned char* __restrict__ dst, const unsigned char* __restri
 }
 
 // ---------------------------------------------------------------------------------------------
-// Allreduce, LL (low latency) -- EXPERIMENTAL, written at the end of round 1: bit-exact against the
-// oracle in worlds of 2 and 4 ranks sharing one B200 (tests/test_gpu_worlds.py::test_ll_...), but
-// its latency over NVLink has not been measured yet, so it is off unless "ll_max_bytes" > 0 or
-// the algorithm is forced.
+// Allreduce, LL (low latency): bit-exact against the oracle in worlds of 2 and 4 ranks sharing one
+// H100 (tests/test_gpu_worlds.py::test_ll_...); its latency over NVLink has not been measured on
+// H100.  AUTO uses it on multi-GPU worlds up to "ll_max_bytes".
 // One kernel, no barrier at all.  Every rank pushes its whole (<= 32 KiB) message into a private
 // lane of every peer's heap as 16-byte cells {data32, seq, data32, seq} (the NCCL "LL" layout: each
 // 8-byte half carries its own flag, so only 8-byte store atomicity is assumed), then reduces its

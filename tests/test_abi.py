@@ -51,10 +51,10 @@ def test_no_link_time_dependency_on_libcuda_or_torch():
     assert "libcuda.so" not in out and "torch" not in out and "nccl" not in out
 
 
-def test_library_contains_sm_100a_code_only():
+def test_library_contains_sm_90a_code_only():
     out = subprocess.run(["cuobjdump", "--list-elf", mpi.LIB_PATH], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_(\d+a?)", out))
-    assert archs == {"100a"}, archs
+    assert archs == {"90a"}, archs
 
 
 def test_before_init_matches_reference_conventions():

@@ -2,7 +2,7 @@
 gloo between rank processes, the oracle's reduction orders) for a world of 1 and a world of 2 -- the
 parity bookkeeping over whole buffers, the contract line and its extra objects, exit codes, and the
 deadline that prints a partial line instead of losing the run.  No kernel runs here; the GPU suite and
-the bench itself on a B200 box cover the product."""
+the bench itself on an H100 cover the product."""
 import json
 import os
 import socket
@@ -114,3 +114,28 @@ def test_bench_deadline_prints_a_partial_line():
     for k in REQUIRED:
         assert k in d, k
     assert "partial line" in d["config"]["note"] and d["value"] > 0
+
+
+def test_bench_dump_outputs(tmp_path):
+    """--dump-outputs DIR: the recv buffer of the last timed step as float32, whole when it is small,
+    else one element per stratum of DUMP_MAX_ELEMS equal strata; in a world of 1 it equals the input."""
+    import numpy as np
+    import bench
+    from oracle import oracle as O
+    for nbytes in (1 << 20, 4 * bench.DUMP_MAX_ELEMS * 2):
+        d = tmp_path / str(nbytes)
+        (rc, out, err), = run_bench(1, "--bytes", str(nbytes), "--steps", "2", "--warmup", "3", "--no-parity", "--no-e2e", "--no-cpu-baseline",
+                                    "--dump-outputs", str(d))
+        assert rc == 0, err[-3000:]
+        assert contract_line(out)["steps"] == 2
+        assert [p.name for p in d.iterdir()] == ["allreduce_recv.npy"]
+        got = np.load(d / "allreduce_recv.npy")
+        count = nbytes // 4
+        want = O.fill_at(np.float32, bench.SEED, 0, count)
+        assert got.dtype == np.float32 and got.nbytes <= 64 << 20
+        if count <= bench.DUMP_MAX_ELEMS:
+            assert np.array_equal(got, want)
+        else:
+            assert got.size == bench.DUMP_MAX_ELEMS
+            strata = want[: got.size * (count // got.size)].reshape(got.size, -1)
+            assert bool((strata == got[:, None]).any(axis=1).all())

@@ -93,7 +93,7 @@ def test_ownership_arithmetic_unit():
     vector owned exactly once for every (count, block shift, world size); LL lane layout."""
     import tempfile
     exe = os.path.join(tempfile.mkdtemp(prefix="b200mpi-owner-"), "owner_test")
-    subprocess.check_call(["/usr/local/cuda/bin/nvcc", "-std=c++17", "-O1", "-gencode", "arch=compute_100a,code=sm_100a", "-o", exe,
+    subprocess.check_call(["/usr/local/cuda/bin/nvcc", "-std=c++17", "-O1", "-gencode", "arch=compute_90a,code=sm_90a", "-o", exe,
                            os.path.join(ROOT, "tests", "cpp", "owner_test.cu"), "-cudart", "static"])
     out = subprocess.run([exe], capture_output=True, text=True, timeout=300)
     assert out.returncode == 0 and "owner ok" in out.stdout, out.stdout + out.stderr

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: pytest -m gpu).  Every test launches a world of rank
+"""GPU parity tests (run on an H100: pytest -m gpu).  Every test launches a world of rank
 processes through the gompirun-style launcher and drives the product through the public API /
 C ABI; results are compared with the CPU oracle on the same seeded inputs.  When the box has fewer
 GPUs than ranks, ranks share device 0 (the kernels and the peer mappings are the same; the GPU

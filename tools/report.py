@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Turn tools/sweep.py JSON lines into markdown tables (bus bandwidth GB/s and time us per size).
 
-    python tools/report.py profiles/r01/sweep_n8_auto_v2.jsonl [more.jsonl ...] [--coll allreduce]
+    python tools/report.py sweep_n8.jsonl [more.jsonl ...] [--coll allreduce]
 
 One table per (file, collective): rows = message size, columns = algorithm (and parameter set / block
 cap when a sweep varied them).  Values failing the sweep's own result check are marked with '!'.

@@ -392,6 +392,264 @@ func (c *Cuda) Wait(destination, tag int) error {
 	return nil
 }
 
+// resized points the receiver at n elements: a slice behind a pointer is re-sliced when its array
+// is large enough and replaced otherwise (as Receive does); a *DeviceSlice must hold n already.
+func resized(what string, recv interface{}, n int) (interface{}, error) {
+	switch v := recv.(type) {
+	case *[]float64:
+		if cap(*v) < n {
+			*v = make([]float64, n)
+		}
+		*v = (*v)[:n]
+		return *v, nil
+	case *[]float32:
+		if cap(*v) < n {
+			*v = make([]float32, n)
+		}
+		*v = (*v)[:n]
+		return *v, nil
+	case *[]int64:
+		if cap(*v) < n {
+			*v = make([]int64, n)
+		}
+		*v = (*v)[:n]
+		return *v, nil
+	case *[]byte:
+		if cap(*v) < n {
+			*v = make([]byte, n)
+		}
+		*v = (*v)[:n]
+		return *v, nil
+	case *Raw:
+		if cap(*v) < n {
+			*v = make(Raw, n)
+		}
+		*v = (*v)[:n]
+		return *v, nil
+	case *DeviceSlice:
+		if v.Len != n {
+			return nil, fmt.Errorf("mpi: %s recv must hold %d elements", what, n)
+		}
+		return v, nil
+	}
+	return nil, fmt.Errorf("mpi: %s needs a pointer to []float64, []float32, []int64, []byte or Raw, or a *DeviceSlice, got %T", what, recv)
+}
+
+// table checks counts against Size() and returns it as the C array.
+func (c *Cuda) table(what string, counts []int) ([]C.size_t, int, error) {
+	if len(counts) != c.Size() {
+		return nil, 0, fmt.Errorf("mpi: %s counts must hold Size() entries", what)
+	}
+	t := make([]C.size_t, len(counts))
+	total := 0
+	for i, n := range counts {
+		if n < 0 {
+			return nil, 0, fmt.Errorf("mpi: %s counts must not be negative", what)
+		}
+		t[i] = C.size_t(n)
+		total += n
+	}
+	return t, total, nil
+}
+
+// lengths is every rank's element count, through one int64 Allgather.
+func (c *Cuda) lengths(n int) ([]int, error) {
+	all := make([]int64, c.Size())
+	if err := c.Allgather([]int64{int64(n)}, all); err != nil {
+		return nil, err
+	}
+	out := make([]int, len(all))
+	for i, v := range all {
+		out[i] = int(v)
+	}
+	return out, nil
+}
+
+func (c *Cuda) Gather(send, recv interface{}, root int) error {
+	sp, sn, sdt, sk, err := lowerTyped("Gather", send)
+	if err != nil {
+		return err
+	}
+	var rp unsafe.Pointer
+	if c.Rank() == root {
+		r, err := resized("Gather", recv, sn*c.Size())
+		if err != nil {
+			return err
+		}
+		var rdt, rk C.int
+		if rp, _, rdt, rk, err = lowerTyped("Gather", r); err != nil {
+			return err
+		}
+		if sdt != rdt || sk != rk {
+			return errors.New("mpi: Gather send and recv must have the same type and memory kind")
+		}
+	}
+	if rc := C.b200mpi_gather(sp, rp, C.size_t(sn), sdt, C.int(root), sk); rc != 0 {
+		return lastError(rc, 0)
+	}
+	return nil
+}
+
+func (c *Cuda) Scatter(send, recv interface{}, root int) error {
+	var sp unsafe.Pointer
+	var sn int
+	var sdt, sk C.int
+	var err error
+	r := recv
+	if c.Rank() == root {
+		if sp, sn, sdt, sk, err = lowerTyped("Scatter", send); err != nil {
+			return err
+		}
+		if sn%c.Size() != 0 {
+			return errors.New("mpi: Scatter send must hold Size() equal blocks")
+		}
+		if r, err = resized("Scatter", recv, sn/c.Size()); err != nil {
+			return err
+		}
+	} else if r, err = resized("Scatter", recv, lenOf(recv)); err != nil {
+		return err
+	}
+	rp, rn, rdt, rk, err := lowerTyped("Scatter", r)
+	if err != nil {
+		return err
+	}
+	if c.Rank() == root && (sdt != rdt || sk != rk) {
+		return errors.New("mpi: Scatter send and recv must have the same type and memory kind")
+	}
+	if rc := C.b200mpi_scatter(sp, rp, C.size_t(rn), rdt, C.int(root), rk); rc != 0 {
+		return lastError(rc, 0)
+	}
+	return nil
+}
+
+// lenOf is the current length of the slice (or DeviceSlice) recv points to.
+func lenOf(recv interface{}) int {
+	switch v := recv.(type) {
+	case *[]float64:
+		return len(*v)
+	case *[]float32:
+		return len(*v)
+	case *[]int64:
+		return len(*v)
+	case *[]byte:
+		return len(*v)
+	case *Raw:
+		return len(*v)
+	case *DeviceSlice:
+		return v.Len
+	}
+	return 0
+}
+
+func (c *Cuda) gatherv(what string, send, recv interface{}, counts []int, root int, all bool) ([]int, error) {
+	sp, sn, sdt, sk, err := lowerTyped(what, send)
+	if err != nil {
+		return nil, err
+	}
+	if counts == nil {
+		if counts, err = c.lengths(sn); err != nil {
+			return nil, err
+		}
+	}
+	t, total, err := c.table(what, counts)
+	if err != nil {
+		return nil, err
+	}
+	if counts[c.Rank()] != sn {
+		return nil, fmt.Errorf("mpi: %s counts[Rank()] must equal len(send)", what)
+	}
+	var rp unsafe.Pointer
+	if all || c.Rank() == root {
+		r, err := resized(what, recv, total)
+		if err != nil {
+			return nil, err
+		}
+		var rdt, rk C.int
+		if rp, _, rdt, rk, err = lowerTyped(what, r); err != nil {
+			return nil, err
+		}
+		if sdt != rdt || sk != rk {
+			return nil, fmt.Errorf("mpi: %s send and recv must have the same type and memory kind", what)
+		}
+	}
+	var rc C.int
+	if all {
+		rc = C.b200mpi_allgatherv(sp, rp, &t[0], sdt, sk)
+	} else {
+		rc = C.b200mpi_gatherv(sp, rp, &t[0], sdt, C.int(root), sk)
+	}
+	if rc != 0 {
+		return nil, lastError(rc, 0)
+	}
+	return counts, nil
+}
+
+func (c *Cuda) Gatherv(send, recv interface{}, counts []int, root int) ([]int, error) {
+	return c.gatherv("Gatherv", send, recv, counts, root, false)
+}
+
+func (c *Cuda) Allgatherv(send, recv interface{}, counts []int) ([]int, error) {
+	return c.gatherv("Allgatherv", send, recv, counts, 0, true)
+}
+
+// Scatterv: root always sends its table with one small Bcast, so the other ranks may pass nil.
+func (c *Cuda) Scatterv(send, recv interface{}, counts []int, root int) ([]int, error) {
+	n, isRoot := c.Size(), c.Rank() == root
+	var sp unsafe.Pointer
+	var sn int
+	var sdt, sk C.int
+	var err error
+	if isRoot {
+		if sp, sn, sdt, sk, err = lowerTyped("Scatterv", send); err != nil {
+			return nil, err
+		}
+		if counts == nil {
+			return nil, errors.New("mpi: Scatterv needs counts on root")
+		}
+	}
+	if counts != nil {
+		if _, total, err := c.table("Scatterv", counts); err != nil {
+			return nil, err
+		} else if isRoot && total != sn {
+			return nil, errors.New("mpi: Scatterv send must hold sum(counts) elements on root")
+		}
+	}
+	rootTable := make([]int64, n)
+	if isRoot {
+		for i, v := range counts {
+			rootTable[i] = int64(v)
+		}
+	}
+	if err := c.Bcast(rootTable, root); err != nil {
+		return nil, err
+	}
+	if counts == nil { // a table that differs from root's fails as ERR_PEER on every rank
+		counts = make([]int, n)
+		for i, v := range rootTable {
+			counts[i] = int(v)
+		}
+	}
+	t, _, err := c.table("Scatterv", counts)
+	if err != nil {
+		return nil, err
+	}
+	r, err := resized("Scatterv", recv, counts[c.Rank()])
+	if err != nil {
+		return nil, err
+	}
+	rp, _, rdt, rk, err := lowerTyped("Scatterv", r)
+	if err != nil {
+		return nil, err
+	}
+	if isRoot && (sdt != rdt || sk != rk) {
+		return nil, errors.New("mpi: Scatterv send and recv must have the same type and memory kind")
+	}
+	if rc := C.b200mpi_scatterv(sp, rp, &t[0], rdt, C.int(root), rk); rc != 0 {
+		return nil, lastError(rc, 0)
+	}
+	return counts, nil
+}
+
 func (c *Cuda) Barrier() error {
 	if rc := C.b200mpi_barrier(); rc != 0 {
 		return lastError(rc, 0)

@@ -24,6 +24,8 @@
 //	Allgather  concatenation in rank order on every rank
 //	Barrier    rendezvous of all ranks
 //	ReduceScatter, Reduce, Alltoall   the usual MPI companions of the above
+//	Gather, Scatter                   rooted collection and distribution of equal blocks
+//	Gatherv, Scatterv, Allgatherv     the same with a different length on every rank
 //	Isend + Wait   the non-blocking Send design the reference sketches and comments out (mpi.go:132-152)
 //
 // They are served through the optional Collective interface, the upgrade the reference hints at
@@ -66,6 +68,18 @@ type Collective2 interface {
 	Alltoall(send, recv interface{}) error
 	Isend(data interface{}, destination, tag int) error
 	Wait(destination, tag int) error
+}
+
+// Collective3 is the third optional upgrade: the rooted and variable-count collectives. Receivers
+// are pointers to slices, resized the way Receive resizes (or a *DeviceSlice of the right length).
+// counts is the same table on every rank; a nil counts is learnt (see Gatherv, Scatterv) and the
+// table used is returned.
+type Collective3 interface {
+	Gather(send, recv interface{}, root int) error
+	Scatter(send, recv interface{}, root int) error
+	Gatherv(send, recv interface{}, counts []int, root int) ([]int, error)
+	Scatterv(send, recv interface{}, counts []int, root int) ([]int, error)
+	Allgatherv(send, recv interface{}, counts []int) ([]int, error)
 }
 
 // Raw marks a payload that is sent as bytes without any encoding.
@@ -229,4 +243,60 @@ func Wait(destination, tag int) error {
 		return err
 	}
 	return c.Wait(destination, tag)
+}
+
+func collective3() (Collective3, error) {
+	if c, ok := current.(Collective3); ok {
+		return c, nil
+	}
+	return nil, fmt.Errorf("mpi: registered implementation %T has no Gather/Scatter/Gatherv/Scatterv/Allgatherv", current)
+}
+
+// Gather stores rank r's send in block r of root's recv, which is resized to Size()*len(send).
+// recv may be nil on the other ranks.
+func Gather(send, recv interface{}, root int) error {
+	c, err := collective3()
+	if err != nil {
+		return err
+	}
+	return c.Gather(send, recv, root)
+}
+
+// Scatter sends block r of root's send (Size() equal blocks) to rank r's recv. root's recv is
+// resized to one block; the other ranks' recv must already hold that length. send may be nil off root.
+func Scatter(send, recv interface{}, root int) error {
+	c, err := collective3()
+	if err != nil {
+		return err
+	}
+	return c.Scatter(send, recv, root)
+}
+
+// Gatherv stores rank r's send at offset counts[0]+...+counts[r-1] of root's recv, resized to
+// sum(counts). A nil counts on every rank is learnt with one Allgather of the lengths.
+func Gatherv(send, recv interface{}, counts []int, root int) ([]int, error) {
+	c, err := collective3()
+	if err != nil {
+		return nil, err
+	}
+	return c.Gatherv(send, recv, counts, root)
+}
+
+// Scatterv sends root's send[displ[r]:displ[r]+counts[r]] to rank r's recv, resized to counts[r].
+// root passes counts; the other ranks may pass nil and learn root's table.
+func Scatterv(send, recv interface{}, counts []int, root int) ([]int, error) {
+	c, err := collective3()
+	if err != nil {
+		return nil, err
+	}
+	return c.Scatterv(send, recv, counts, root)
+}
+
+// Allgatherv is Gatherv with the result on every rank.
+func Allgatherv(send, recv interface{}, counts []int) ([]int, error) {
+	c, err := collective3()
+	if err != nil {
+		return nil, err
+	}
+	return c.Allgatherv(send, recv, counts)
 }

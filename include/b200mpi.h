@@ -30,7 +30,8 @@
 extern "C" {
 #endif
 
-#define B200MPI_VERSION 200 /* 0.2.0: + isend/wait, reduce_scatter, reduce, alltoall, probes, get_param (additive) */
+#define B200MPI_VERSION 200 /* 0.2.0: + isend/wait, reduce_scatter, reduce, alltoall, probes, get_param;
+                               then gather, scatter, gatherv, scatterv, allgatherv (all additive) */
 #define B200MPI_MAX_RANKS 8 /* "the 8 GPUs of one box" */
 
 typedef enum {
@@ -146,6 +147,20 @@ int b200mpi_reduce_scatter(const void* send, void* recv, size_t count_per_rank, 
 int b200mpi_reduce(const void* send, void* recv, size_t count, int dtype, int op, int root, int memkind);
 /* send and recv hold size()*count_per_rank elements; block j of send becomes block rank() of rank j's recv. */
 int b200mpi_alltoall(const void* send, void* recv, size_t count_per_rank, int dtype, int memkind);
+/* recv (root only, may be NULL elsewhere) holds size()*count_per_rank; rank r's send lands at r*count_per_rank.
+ * In place on root: send == recv + root*count_per_rank. */
+int b200mpi_gather(const void* send, void* recv, size_t count_per_rank, int dtype, int root, int memkind);
+/* send (root only, may be NULL elsewhere) holds size()*count_per_rank; block r goes to rank r's recv.
+ * In place on root: recv == send + root*count_per_rank. */
+int b200mpi_scatter(const void* send, void* recv, size_t count_per_rank, int dtype, int root, int memkind);
+/* counts[size()]: the same table on every rank (a rank whose table differs gets B200MPI_ERR_PEER, as
+ * do all others).  Blocks are packed in rank order: displacement of rank r = counts[0] + ... +
+ * counts[r-1] elements.  Any count may be 0.  In place: gatherv on root send == recv + displ[root],
+ * scatterv on root recv == send + displ[root], allgatherv send == recv + displ[rank()].  Buffers
+ * that are not in the b200mpi_alloc heap are staged whole through it (B200MPI_ERR_NOMEM if too big). */
+int b200mpi_gatherv(const void* send, void* recv, const size_t* counts, int dtype, int root, int memkind);
+int b200mpi_scatterv(const void* send, void* recv, const size_t* counts, int dtype, int root, int memkind);
+int b200mpi_allgatherv(const void* send, void* recv, const size_t* counts, int dtype, int memkind);
 int b200mpi_barrier(void);
 
 /* Enqueue-only forms on the library stream (DEVICE memkind only). */

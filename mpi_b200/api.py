@@ -6,6 +6,8 @@ Same names, same argument meaning, same blocking behaviour:
     Register(impl)  Interface  Raw  TagExists                       (the reference's surface)
     Recv  Bcast(data, root)  Allreduce(send, recv, op)  Allgather(send, recv)  Barrier()   (new)
     ReduceScatter(send, recv, op)  Reduce(send, recv, op, root)  Alltoall(send, recv)      (new)
+    Gather(send, recv, root)  Scatter(send, recv, root)                                       (new)
+    Gatherv(send, recv, root, counts)  Scatterv(send, recv, counts, root)  Allgatherv(send, recv, counts)
     Isend(data, destination, tag) + Wait(destination, tag)     (the Send/Wait design commented out
                                                                 in the reference, mpi.go:132-152)
 
@@ -305,6 +307,134 @@ class Cuda(Interface):
     def Barrier(self):
         _check(L.load().b200mpi_barrier())
 
+    # -- rooted and variable-count collectives ----------------------------------------------------
+    def _world(self):
+        n = self.Size()
+        if n <= 0:
+            raise MpiError(L.ERR_NOT_INIT, "mpi: Init has not been called")
+        return self.Rank(), n
+
+    def Gather(self, send, recv, root):
+        """Rank r's send lands in block r of root's recv (Size()*len(send) elements); recv is
+        ignored and may be None off root.  In place on root: send is root's block of recv."""
+        rank, n = self._world()
+        sp, sc, sdt, sk, keep, _ = _describe(send)  # keep: a str travels as a temporary encoding
+        rp = None
+        if rank == root:
+            if recv is None:
+                raise ValueError("mpi: Gather needs a recv buffer on root")
+            rp, rc_, rdt, rk, _, _ = _describe(recv)
+            if rc_ != sc * n or sdt != rdt or sk != rk:
+                raise ValueError("mpi: Gather recv must hold Size()*len(send) elements of the same type and memory kind")
+        _check(L.load().b200mpi_gather(sp, rp, sc, sdt, int(root), sk))
+        return recv
+
+    def Scatter(self, send, recv, root):
+        """Block r of root's send (Size()*len(recv) elements) goes to rank r's recv; send is
+        ignored and may be None off root.  In place on root: recv is root's block of send."""
+        rank, n = self._world()
+        rp, rc_, rdt, rk, _, _ = _describe(recv)
+        sp = None
+        if rank == root:
+            if send is None:
+                raise ValueError("mpi: Scatter needs a send buffer on root")
+            sp, sc, sdt, sk, keep, _ = _describe(send)
+            if sc != rc_ * n or sdt != rdt or sk != rk:
+                raise ValueError("mpi: Scatter send must hold Size()*len(recv) elements of the same type and memory kind")
+        _check(L.load().b200mpi_scatter(sp, rp, rc_, rdt, int(root), rk))
+        return recv
+
+    def _table(self, counts, n):
+        counts = [int(c) for c in counts]
+        if len(counts) != n or any(c < 0 for c in counts):
+            raise ValueError("mpi: counts must hold Size() non-negative element counts")
+        return counts, (ctypes.c_size_t * n)(*counts)
+
+    def _lengths(self, count):
+        """Every rank's element count, through one int64 Allgather."""
+        n = self.Size()
+        mine = np.array([count], dtype=np.int64)
+        everyone = np.empty(n, dtype=np.int64)
+        self.Allgather(mine, everyone)
+        return everyone.tolist()
+
+    @staticmethod
+    def _recv_for(recv, total, dt, kind, what):
+        """recv of `total` elements: a host array that is missing or too small is replaced by a new one
+        (as Receive resizes), a larger one is used through a view of the right length."""
+        if recv is None:
+            if kind != L.HOST:
+                raise ValueError("mpi: %s needs a recv DeviceSlice for a DeviceSlice send" % what)
+            recv = np.empty(total, dtype=_DT2NP[dt])
+        rp, rc_, rdt, rk, _, _ = _describe(recv)
+        if rdt != dt or rk != kind:
+            raise ValueError("mpi: %s send and recv must have the same type and memory kind" % what)
+        if rc_ != total:
+            if rk != L.HOST or not isinstance(recv, np.ndarray):
+                raise ValueError("mpi: %s recv must hold %d elements" % (what, total))
+            recv = np.empty(total, dtype=_DT2NP[dt]) if rc_ < total else recv.reshape(-1)[:total]
+            rp = recv.ctypes.data if total else None
+        return recv, rp
+
+    def Gatherv(self, send, recv=None, root=0, counts=None):
+        """Rank r's send lands at displacement counts[0]+...+counts[r-1] of root's recv.  counts is
+        the same table on every rank; omitted on every rank, it is learnt with one Allgather.
+        Returns (recv, counts); off root recv is returned as passed."""
+        rank, n = self._world()
+        sp, sc, sdt, sk, keep, _ = _describe(send)
+        if counts is None:
+            counts = self._lengths(sc)
+        counts, table = self._table(counts, n)
+        if counts[rank] != sc:
+            raise ValueError("mpi: Gatherv counts[Rank()] must equal len(send)")
+        rp = None
+        if rank == root:
+            recv, rp = self._recv_for(recv, sum(counts), sdt, sk, "Gatherv")
+        _check(L.load().b200mpi_gatherv(sp, rp, table, sdt, int(root), sk))
+        return recv, counts
+
+    def Allgatherv(self, send, recv=None, counts=None):
+        """Rank r's send lands at displacement counts[0]+...+counts[r-1] of every rank's recv.
+        counts as for Gatherv.  Returns (recv, counts)."""
+        rank, n = self._world()
+        sp, sc, sdt, sk, keep, _ = _describe(send)
+        if counts is None:
+            counts = self._lengths(sc)
+        counts, table = self._table(counts, n)
+        if counts[rank] != sc:
+            raise ValueError("mpi: Allgatherv counts[Rank()] must equal len(send)")
+        recv, rp = self._recv_for(recv, sum(counts), sdt, sk, "Allgatherv")
+        _check(L.load().b200mpi_allgatherv(sp, rp, table, sdt, sk))
+        return recv, counts
+
+    def Scatterv(self, send, recv, counts=None, root=0):
+        """Block r of root's send, at displacement counts[0]+...+counts[r-1], goes to rank r's recv.
+        Root passes counts; the other ranks may pass None and learn root's table, which root always
+        sends with one small Bcast.  A host recv that is too small is replaced as in Gatherv; recv
+        gives the element type, so it is needed on every rank.  Returns (recv, counts)."""
+        rank, n = self._world()
+        if recv is None:
+            raise ValueError("mpi: Scatterv needs a recv buffer (or an empty array of the element type)")
+        _, rc_, rdt, rk, _, _ = _describe(recv)
+        sp = None
+        if rank == root:
+            if send is None or counts is None:
+                raise ValueError("mpi: Scatterv needs send and counts on root")
+            sp, sc, sdt, sk, keep, _ = _describe(send)
+            counts, _ = self._table(counts, n)
+            if sum(counts) != sc or sdt != rdt or sk != rk:
+                raise ValueError("mpi: Scatterv send must hold sum(counts) elements of recv's type and memory kind")
+        elif counts is not None:
+            counts, _ = self._table(counts, n)
+        root_table = np.array(counts if rank == root else [0] * n, dtype=np.int64)
+        self.Bcast(root_table, root)
+        if counts is None:
+            counts = root_table.tolist()
+        counts, table = self._table(counts, n)  # a table that differs from root's fails as ERR_PEER on every rank
+        recv, rp = self._recv_for(recv, counts[rank], rdt, rk, "Scatterv")
+        _check(L.load().b200mpi_scatterv(sp, rp, table, rdt, int(root), rk))
+        return recv, counts
+
 
 # ---- package-level facade: mpi.go:56-159 -------------------------------------------------------
 _mpier = Cuda()
@@ -386,6 +516,26 @@ def Reduce(send, recv, op=SUM, root=0):
 
 def Alltoall(send, recv):
     return _collective("Alltoall")(send, recv)
+
+
+def Gather(send, recv, root):
+    return _collective("Gather")(send, recv, root)
+
+
+def Scatter(send, recv, root):
+    return _collective("Scatter")(send, recv, root)
+
+
+def Gatherv(send, recv=None, root=0, counts=None):
+    return _collective("Gatherv")(send, recv, root, counts)
+
+
+def Scatterv(send, recv, counts=None, root=0):
+    return _collective("Scatterv")(send, recv, counts, root)
+
+
+def Allgatherv(send, recv=None, counts=None):
+    return _collective("Allgatherv")(send, recv, counts)
 
 
 def Isend(data, destination, tag):

@@ -13,7 +13,8 @@
 //   mpi.Receive(&data, src, tag)               mpi::Error mpi::Receive(T* data, int src, int tag)   (resizes *data like gob)
 //   mpi.Register(impl)                         void mpi::Register(Interface*)  (second call throws = panics, mpi.go:61-67)
 //   flag.Parse() + mpi.Flag*                   mpi::ParseFlags(argc, argv) + mpi::Flag*
-//   new: Recv, Bcast, Allreduce, Allgather, Barrier, ReduceScatter, Reduce, Alltoall, Isend/Wait;
+//   new: Recv, Bcast, Allreduce, Allgather, Barrier, ReduceScatter, Reduce, Alltoall, Isend/Wait,
+//        Gather, Scatter, Gatherv, Scatterv, Allgatherv;
 //        mpi::DeviceSlice<T> for heap-resident buffers
 // `data` may be std::vector<double|float|int64_t|uint8_t>, std::string (sent as bytes, the
 // "anything else is gob-encoded" path), or DeviceSlice<T>.
@@ -174,6 +175,12 @@ struct Interface {
   virtual Error ReduceScatter(Buffer, Buffer, Op) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no ReduceScatter"; return e; }
   virtual Error Reduce(Buffer, Buffer, Op, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Reduce"; return e; }
   virtual Error Alltoall(Buffer, Buffer) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Alltoall"; return e; }
+  // rooted and variable-count collectives: counts[Size()] is the same table on every rank
+  virtual Error Gather(Buffer, Buffer, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Gather"; return e; }
+  virtual Error Scatter(Buffer, Buffer, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Scatter"; return e; }
+  virtual Error Gatherv(Buffer, Buffer, const size_t*, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Gatherv"; return e; }
+  virtual Error Scatterv(Buffer, Buffer, const size_t*, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Scatterv"; return e; }
+  virtual Error Allgatherv(Buffer, Buffer, const size_t*) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Allgatherv"; return e; }
   // the Send/Wait pair the reference sketches and comments out (mpi.go:132-152)
   virtual Error Isend(Buffer, int, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Isend"; return e; }
   virtual Error Wait(int, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Wait"; return e; }
@@ -208,6 +215,11 @@ struct Cuda : Interface {
   Error ReduceScatter(Buffer s, Buffer r, Op op) override { return make_error(b200mpi_reduce_scatter(s.ptr, r.ptr, r.count, s.dtype, op, s.memkind)); }
   Error Reduce(Buffer s, Buffer r, Op op, int root) override { return make_error(b200mpi_reduce(s.ptr, r.ptr, s.count, s.dtype, op, root, s.memkind)); }
   Error Alltoall(Buffer s, Buffer r) override { return make_error(b200mpi_alltoall(s.ptr, r.ptr, s.count / (size_t)(Size() > 0 ? Size() : 1), s.dtype, s.memkind)); }
+  Error Gather(Buffer s, Buffer r, int root) override { return make_error(b200mpi_gather(s.ptr, r.ptr, s.count, s.dtype, root, s.memkind)); }
+  Error Scatter(Buffer s, Buffer r, int root) override { return make_error(b200mpi_scatter(s.ptr, r.ptr, r.count, r.dtype, root, r.memkind)); }
+  Error Gatherv(Buffer s, Buffer r, const size_t* counts, int root) override { return make_error(b200mpi_gatherv(s.ptr, r.ptr, counts, s.dtype, root, s.memkind)); }
+  Error Scatterv(Buffer s, Buffer r, const size_t* counts, int root) override { return make_error(b200mpi_scatterv(s.ptr, r.ptr, counts, r.dtype, root, r.memkind)); }
+  Error Allgatherv(Buffer s, Buffer r, const size_t* counts) override { return make_error(b200mpi_allgatherv(s.ptr, r.ptr, counts, s.dtype, s.memkind)); }
   Error Isend(Buffer d, int destination, int tag) override { return make_error(b200mpi_isend(d.ptr, d.count, d.dtype, destination, tag, d.memkind)); }
   Error Wait(int destination, int tag) override { return make_error(b200mpi_wait(destination, tag)); }
 };
@@ -287,6 +299,68 @@ template <typename T> inline Error Alltoall(const std::vector<T>& send, std::vec
   recv->resize(send.size());
   return mpier()->Alltoall(lower(send), lower(*recv));
 }
+
+// Gather: root's recv is resized to Size() blocks of len(send).  Scatter: root's recv is resized to
+// one block of send; elsewhere recv must already hold that block length.
+template <typename T> inline Error Gather(const std::vector<T>& send, std::vector<T>* recv, int root) {
+  if (Rank() == root) recv->resize(send.size() * (size_t)Size());
+  return mpier()->Gather(lower(send), lower(*recv), root);
+}
+template <typename T> inline Error Gather(const DeviceSlice<T>& send, DeviceSlice<T>* recv, int root) { return mpier()->Gather(lower(send), lower(*recv), root); }
+template <typename T> inline Error Scatter(const std::vector<T>& send, std::vector<T>* recv, int root) {
+  if (Rank() == root && Size() > 0) recv->resize(send.size() / (size_t)Size());
+  return mpier()->Scatter(lower(send), lower(*recv), root);
+}
+template <typename T> inline Error Scatter(const DeviceSlice<T>& send, DeviceSlice<T>* recv, int root) { return mpier()->Scatter(lower(send), lower(*recv), root); }
+
+inline Error arg_error(const std::string& msg) { Error e; e.code = B200MPI_ERR_ARG; e.msg = msg; return e; }
+// An empty *counts is filled with every rank's len(send) through one int64 Allgather; a given one
+// must hold Size() entries with counts[Rank()] == len(send).
+inline Error fill_counts(size_t mine, std::vector<size_t>* counts, const char* what) {
+  const size_t n = (size_t)(Size() > 0 ? Size() : 0);
+  if (counts->empty() && n > 0) {
+    std::vector<int64_t> one(1, (int64_t)mine), all;
+    Error e = Allgather(one, &all);
+    if (e) return e;
+    counts->assign(all.begin(), all.end());
+  }
+  if (n > 0 && counts->size() != n) return arg_error(std::string("mpi: ") + what + " counts must hold Size() entries");
+  if (n > 0 && (*counts)[(size_t)Rank()] != mine) return arg_error(std::string("mpi: ") + what + " counts[Rank()] must equal len(send)");
+  return {};
+}
+inline size_t sum_of(const std::vector<size_t>& c) { size_t s = 0; for (size_t x : c) s += x; return s; }
+
+// Gatherv / Allgatherv: root's (every rank's) recv is resized to sum(counts), as Receive resizes.
+template <typename T> inline Error Gatherv(const std::vector<T>& send, std::vector<T>* recv, int root, std::vector<size_t>* counts) {
+  Error e = fill_counts(send.size(), counts, "Gatherv");
+  if (e) return e;
+  if (Rank() == root) recv->resize(sum_of(*counts));
+  return mpier()->Gatherv(lower(send), lower(*recv), counts->data(), root);
+}
+template <typename T> inline Error Allgatherv(const std::vector<T>& send, std::vector<T>* recv, std::vector<size_t>* counts) {
+  Error e = fill_counts(send.size(), counts, "Allgatherv");
+  if (e) return e;
+  recv->resize(sum_of(*counts));
+  return mpier()->Allgatherv(lower(send), lower(*recv), counts->data());
+}
+// Scatterv: root passes the table; root always sends it with one small Bcast, so the other ranks
+// may pass an empty *counts and learn it.  recv is resized to counts[Rank()].
+template <typename T> inline Error Scatterv(const std::vector<T>& send, std::vector<T>* recv, std::vector<size_t>* counts, int root) {
+  const size_t n = (size_t)(Size() > 0 ? Size() : 0);
+  const bool is_root = Rank() == root;
+  if (n > 0 && ((is_root || !counts->empty()) && counts->size() != n)) return arg_error("mpi: Scatterv counts must hold Size() entries (root must pass them)");
+  if (n > 0 && is_root && sum_of(*counts) != send.size()) return arg_error("mpi: Scatterv send must hold sum(counts) elements on root");
+  if (n > 0) {
+    std::vector<int64_t> table(n, 0);
+    if (is_root) table.assign(counts->begin(), counts->end());
+    Error e = Bcast(&table, root);
+    if (e) return e;
+    if (counts->empty()) counts->assign(table.begin(), table.end()); // a table that differs from root's fails as B200MPI_ERR_PEER
+    recv->resize((*counts)[(size_t)Rank()]);
+  }
+  return mpier()->Scatterv(lower(send), lower(*recv), counts->data(), root);
+}
+
 template <typename D> inline Error Isend(const D& data, int destination, int tag) { return mpier()->Isend(lower(data), destination, tag); }
 inline Error Wait(int destination, int tag) { return mpier()->Wait(destination, tag); }
 

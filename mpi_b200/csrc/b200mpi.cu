@@ -312,7 +312,8 @@ static int check_status() {
 }
 
 // What this rank thinks the call is, folded into one word; equal on every rank of a well-formed
-// call.  coll: 0 allreduce, 1 bcast, 2 allgather, 3 barrier, 4 reduce_scatter, 5 reduce, 6 alltoall.
+// call.  coll: 0 allreduce, 1 bcast, 2 allgather, 3 barrier, 4 reduce_scatter, 5 reduce, 6 alltoall,
+// 7 gather(v), 8 scatter(v), 9 allgatherv (these three carry a hash of the counts table in `total`).
 // `total` is the element count of the whole user call when the launch is one chunk of a pipelined
 // host-slice call (ranks that disagree about the total then disagree from the first chunk on).
 static uint64_t mix64(uint64_t x) {
@@ -1242,6 +1243,142 @@ static int do_alltoall(const void* send, void* recv, size_t count, int dtype, in
 }
 
 // ---------------------------------------------------------------------------------------------
+// Gather(v), Scatter(v), Allgatherv: blocks of counts[r] elements packed in rank order.  One
+// algorithm each, no host pipelining: host slices and foreign device pointers are staged whole.
+// ---------------------------------------------------------------------------------------------
+// counts[n] -> byte displacements, and a hash of the whole table for the call signature (order
+// matters: tables that differ by a swap of two counts hash differently).
+static int make_vtable(const char* what, const size_t* counts, size_t es, VTable& vt, uint64_t& hash) {
+  const int n = g->ctrl.n;
+  if (!counts) return fail(B200MPI_ERR_ARG, std::string(what) + ": NULL counts table");
+  uint64_t off = 0;
+  hash = 0x76746162ull;
+  for (int r = 0; r < n; ++r) {
+    vt.off[r] = off;
+    if (counts[r] > (SIZE_MAX - off) / es) return fail(B200MPI_ERR_ARG, std::string(what) + ": sum(counts) * element size overflows");
+    off += counts[r] * es;
+    hash = mix64(hash ^ (counts[r] + 0x9e3779b97f4a7c15ull * (uint64_t)(r + 1)));
+  }
+  for (int r = n; r <= kMaxRanks; ++r) vt.off[r] = off;
+  return 0;
+}
+
+// which: 0 gather(v) / allgatherv push (peer = destination rank, -1 all), 1 scatterv pull (peer = root).
+// The grid follows the largest block of the table, so every rank launches the same one; the access
+// unit follows this rank's offsets and every displacement (the table is the same everywhere).
+template <typename U>
+static void launch_v_u(int which, Comm& c, uint64_t a, uint64_t b, const VTable& vt, int peer, cudaStream_t s) {
+  constexpr int UNROLL = 4;
+  size_t largest = 0;
+  for (int r = 0; r < c.n; ++r) largest = std::max<size_t>(largest, vt.off[r + 1] - vt.off[r]);
+  const int blocks = grid_for(largest / 16 + 1, UNROLL);
+  sig_grid(c, blocks);
+  if (which == 0) gatherv_push_kernel<U, UNROLL><<<blocks, kThreads, 0, s>>>(c, a, b, vt, peer);
+  else scatterv_pull_kernel<U, UNROLL><<<blocks, kThreads, 0, s>>>(c, a, b, vt, peer);
+}
+static int launch_v(int which, uint64_t a, uint64_t b, const VTable& vt, int peer, cudaStream_t s) {
+  Comm c = next_comm();
+  uint64_t m = a | b;
+  for (int r = 0; r <= c.n; ++r) m |= vt.off[r];
+  if ((m & 15) == 0) launch_v_u<uint4>(which, c, a, b, vt, peer, s);
+  else if ((m & 7) == 0) launch_v_u<unsigned long long>(which, c, a, b, vt, peer, s);
+  else if ((m & 3) == 0) launch_v_u<unsigned int>(which, c, a, b, vt, peer, s);
+  else launch_v_u<unsigned char>(which, c, a, b, vt, peer, s);
+  return launch_check(which == 0 ? "gatherv_push_kernel" : "scatterv_pull_kernel");
+}
+
+// A staged result is copied back only after the collective succeeded: a mismatched call
+// (B200MPI_ERR_PEER) leaves the caller's buffer untouched, as it does for heap buffers.
+static int copy_out_checked(void* p, size_t bytes, int memkind, const Buf& b) {
+  if (!b.staged || bytes == 0) return 0;
+  CUDA_OK(cudaStreamSynchronize(g->stream));
+  int rc = check_status();
+  if (rc) return rc;
+  return copy_out(p, bytes, memkind, b);
+}
+
+static int check_v_args(const char* what, int dtype, int memkind, size_t& es) {
+  es = esize(dtype);
+  if (es == 0) return fail(B200MPI_ERR_ARG, std::string(what) + ": unknown dtype");
+  if (memkind != B200MPI_HOST && memkind != B200MPI_DEVICE) return fail(B200MPI_ERR_ARG, std::string(what) + ": bad memkind");
+  return 0;
+}
+
+// Gatherv: rank r's send lands at displacement r of root's recv; recv may be NULL off root.
+// Allgatherv (all): it lands at displacement r of every rank's recv.
+static int do_gatherv(const void* send, void* recv, const size_t* counts, int dtype, int root, bool all, int memkind) {
+  int rc = need_data_plane();
+  if (rc) return rc;
+  const char* what = all ? "allgatherv" : "gatherv";
+  const int n = g->ctrl.n, me = g->ctrl.rank;
+  size_t es;
+  if ((rc = check_v_args(what, dtype, memkind, es))) return rc;
+  if (all) root = -1;
+  else if (root < 0 || root >= n) return fail(B200MPI_ERR_ARG, "gatherv: root out of range");
+  VTable vt;
+  uint64_t hash;
+  if ((rc = make_vtable(what, counts, es, vt, hash))) return rc;
+  const size_t mine = vt.off[me + 1] - vt.off[me], total = vt.off[n];
+  const bool gets = all || me == root; // this rank's recv is written
+  if ((mine && !send) || (gets && total && !recv)) return fail(B200MPI_ERR_ARG, std::string(what) + ": NULL buffer with count > 0");
+  const bool inplace = gets && recv && (const char*)send == (const char*)recv + vt.off[me];
+  if (n == 1) return local_copy(recv, send, total, memkind, false);
+  Buf in, out;
+  if (gets) {
+    rc = resolve_out(recv, total, memkind, 1, out);
+    if (rc) return rc;
+  }
+  if (inplace && !out.staged) in.off = out.off + vt.off[me];
+  else if ((rc = resolve_in(send, mine, memkind, 0, in))) return rc;
+  if (!gets) out = in; // announced but never written: only root's recv is a destination
+  g->cur_sig = make_sig(all ? 9 : 7, dtype, root, 0, total / es, hash);
+  rc = launch_v(0, in.off, out.off, vt, root, g->stream);
+  if (rc) return rc;
+  if (gets && (rc = copy_out_checked(recv, total, memkind, out))) return rc;
+  return finish(false);
+}
+
+// Scatterv: block r of root's send (NULL allowed off root) goes to rank r's recv.
+static int do_scatterv(const void* send, void* recv, const size_t* counts, int dtype, int root, int memkind) {
+  int rc = need_data_plane();
+  if (rc) return rc;
+  const int n = g->ctrl.n, me = g->ctrl.rank;
+  size_t es;
+  if ((rc = check_v_args("scatterv", dtype, memkind, es))) return rc;
+  if (root < 0 || root >= n) return fail(B200MPI_ERR_ARG, "scatterv: root out of range");
+  VTable vt;
+  uint64_t hash;
+  if ((rc = make_vtable("scatterv", counts, es, vt, hash))) return rc;
+  const size_t mine = vt.off[me + 1] - vt.off[me], total = vt.off[n];
+  const bool is_root = me == root;
+  if ((mine && !recv) || (is_root && total && !send)) return fail(B200MPI_ERR_ARG, "scatterv: NULL buffer with count > 0");
+  if (n == 1) return local_copy(recv, send, total, memkind, false);
+  Buf in, out;
+  if (is_root) {
+    rc = resolve_in(send, total, memkind, 0, in);
+    if (rc) return rc;
+  }
+  const bool inplace = is_root && send && (const char*)recv == (const char*)send + vt.off[me];
+  if (inplace && !in.staged) out.off = in.off + vt.off[me];
+  else if ((rc = resolve_out(recv, mine, memkind, 1, out))) return rc;
+  if (!is_root) in = out; // announced but never read: only root's send is a source
+  g->cur_sig = make_sig(8, dtype, root, 0, total / es, hash);
+  rc = launch_v(1, in.off, out.off, vt, root, g->stream);
+  if (rc) return rc;
+  rc = copy_out_checked(recv, mine, memkind, out);
+  if (rc) return rc;
+  return finish(false);
+}
+
+// The fixed-count forms: the uniform table.
+static int do_gather(const void* send, void* recv, size_t count, int dtype, int root, int memkind, bool scatter) {
+  int rc = need_data_plane();
+  if (rc) return rc;
+  const std::vector<size_t> counts((size_t)g->ctrl.n, count);
+  return scatter ? do_scatterv(send, recv, counts.data(), dtype, root, memkind) : do_gatherv(send, recv, counts.data(), dtype, root, false, memkind);
+}
+
+// ---------------------------------------------------------------------------------------------
 // point to point
 // ---------------------------------------------------------------------------------------------
 static Ctx::P2PBounce* acquire_bounce() {
@@ -1919,6 +2056,11 @@ int b200mpi_allgather(const void* send, void* recv, size_t count, int dtype, int
 int b200mpi_reduce_scatter(const void* send, void* recv, size_t count_per_rank, int dtype, int op, int memkind) { return do_reduce_scatter(send, recv, count_per_rank, dtype, op, memkind, false); }
 int b200mpi_reduce(const void* send, void* recv, size_t count, int dtype, int op, int root, int memkind) { return do_reduce(send, recv, count, dtype, op, root, memkind, false); }
 int b200mpi_alltoall(const void* send, void* recv, size_t count_per_rank, int dtype, int memkind) { return do_alltoall(send, recv, count_per_rank, dtype, memkind, false); }
+int b200mpi_gather(const void* send, void* recv, size_t count_per_rank, int dtype, int root, int memkind) { return do_gather(send, recv, count_per_rank, dtype, root, memkind, false); }
+int b200mpi_scatter(const void* send, void* recv, size_t count_per_rank, int dtype, int root, int memkind) { return do_gather(send, recv, count_per_rank, dtype, root, memkind, true); }
+int b200mpi_gatherv(const void* send, void* recv, const size_t* counts, int dtype, int root, int memkind) { return do_gatherv(send, recv, counts, dtype, root, false, memkind); }
+int b200mpi_scatterv(const void* send, void* recv, const size_t* counts, int dtype, int root, int memkind) { return do_scatterv(send, recv, counts, dtype, root, memkind); }
+int b200mpi_allgatherv(const void* send, void* recv, const size_t* counts, int dtype, int memkind) { return do_gatherv(send, recv, counts, dtype, 0, true, memkind); }
 int b200mpi_reduce_scatter_async(const void* send, void* recv, size_t count_per_rank, int dtype, int op) { return do_reduce_scatter(send, recv, count_per_rank, dtype, op, B200MPI_DEVICE, true); }
 int b200mpi_bcast_async(void* buf, size_t count, int dtype, int root) { return do_bcast(buf, count, dtype, root, B200MPI_DEVICE, true); }
 int b200mpi_allreduce_async(const void* send, void* recv, size_t count, int dtype, int op) { return do_allreduce(send, recv, count, dtype, op, B200MPI_DEVICE, true); }

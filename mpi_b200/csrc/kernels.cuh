@@ -1413,6 +1413,116 @@ alltoall_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t bytes_per_b
 }
 
 // ---------------------------------------------------------------------------------------------
+// Gather(v) / Allgatherv / Scatter(v): blocks of per-rank sizes packed in rank order.  The table is
+// the same on every rank (it is part of the call signature), so only the heap offsets can differ.
+// ---------------------------------------------------------------------------------------------
+struct VTable {
+  uint64_t off[kMaxRanks + 1]; // byte displacement of rank r's block; off[n] = total bytes
+};
+
+// [off[me], off[me+1]) without indexing the parameter array by a runtime value
+__device__ __forceinline__ void vtable_range(const VTable& vt, int me, uint64_t& lo, uint64_t& hi) {
+  lo = 0;
+  hi = 0;
+#pragma unroll
+  for (int r = 0; r < kMaxRanks; ++r)
+    if (r == me) { lo = vt.off[r]; hi = vt.off[r + 1]; }
+}
+
+// Every rank streams its own block once from local HBM and stores it at its displacement in the
+// recv buffer of `only_dst` (Gather) or of all n ranks, own last (only_dst == -1: Allgatherv).  The
+// own copy is skipped when the call is in place (send == recv + displacement).
+template <typename U, int UNROLL>
+__device__ __forceinline__ void gatherv_push_body(const Comm& c, const uint64_t* s_a, const uint64_t* s_b, const VTable& vt, int only_dst) {
+  const int n = c.n;
+  uint64_t lo, hi;
+  vtable_range(vt, c.rank, lo, hi);
+  const size_t units = (hi - lo) / sizeof(U);
+  const U* src = reinterpret_cast<const U*>(c.base[c.rank] + s_a[c.rank]);
+  const bool inplace = s_a[c.rank] == s_b[c.rank] + lo;
+  U* dst[kMaxRanks];
+#pragma unroll
+  for (int r = 0; r < kMaxRanks; ++r) {
+    const int w = only_dst >= 0 ? only_dst : (c.rank + 1 + r) % n; // w == rank when r == n-1
+    dst[r] = reinterpret_cast<U*>(c.base[w] + s_b[w] + lo);
+  }
+  const int ntargets = only_dst >= 0 ? (only_dst == c.rank && inplace ? 0 : 1) : (inplace ? n - 1 : n);
+  const size_t step = (size_t)gridDim.x * blockDim.x * UNROLL;
+  for (size_t i0 = (size_t)blockIdx.x * blockDim.x * UNROLL + threadIdx.x; i0 < units; i0 += step) {
+    U v[UNROLL];
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u) {
+      const size_t i = i0 + (size_t)u * blockDim.x;
+      if (i < units) v[u] = src[i];
+    }
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u) {
+      const size_t i = i0 + (size_t)u * blockDim.x;
+      if (i < units) {
+#pragma unroll
+        for (int r = 0; r < kMaxRanks; ++r)
+          if (r < ntargets) dst[r][i] = v[u];
+      }
+    }
+  }
+}
+
+template <typename U, int UNROLL>
+__global__ void __launch_bounds__(kThreads, 1)
+gatherv_push_kernel(Comm c, uint64_t send_off, uint64_t recv_off, VTable vt, int only_dst) {
+  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
+  const bool call_ok = sync_start(c, send_off, recv_off, s_a, s_b);
+  if (!call_ok) {
+    sync_end_failed(c);
+    return;
+  }
+  if (sizeof(U) == 1 || all_aligned_to(s_a, s_b, c.n, sizeof(U))) gatherv_push_body<U, UNROLL>(c, s_a, s_b, vt, only_dst);
+  else gatherv_push_body<unsigned char, 1>(c, s_a, s_b, vt, only_dst);
+  sync_end(c);
+}
+
+// Every rank pulls its block [off[rank], off[rank+1]) of root's send through the peer mapping into
+// its own recv; root copies its block locally unless the call is in place (recv == send +
+// displacement).  Root's egress bounds it either way; pulling spreads the loads over n-1 GPUs.
+template <typename U, int UNROLL>
+__device__ __forceinline__ void scatterv_pull_body(const Comm& c, const uint64_t* s_a, const uint64_t* s_b, const VTable& vt, int root) {
+  uint64_t lo, hi;
+  vtable_range(vt, c.rank, lo, hi);
+  if (c.rank == root && s_b[root] == s_a[root] + lo) return;
+  const size_t units = (hi - lo) / sizeof(U);
+  const U* src = reinterpret_cast<const U*>(c.base[root] + s_a[root] + lo);
+  U* dst = reinterpret_cast<U*>(c.base[c.rank] + s_b[c.rank]);
+  const size_t step = (size_t)gridDim.x * blockDim.x * UNROLL;
+  for (size_t i0 = (size_t)blockIdx.x * blockDim.x * UNROLL + threadIdx.x; i0 < units; i0 += step) {
+    U v[UNROLL];
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u) {
+      const size_t i = i0 + (size_t)u * blockDim.x;
+      if (i < units) v[u] = src[i];
+    }
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u) {
+      const size_t i = i0 + (size_t)u * blockDim.x;
+      if (i < units) dst[i] = v[u];
+    }
+  }
+}
+
+template <typename U, int UNROLL>
+__global__ void __launch_bounds__(kThreads, 1)
+scatterv_pull_kernel(Comm c, uint64_t send_off, uint64_t recv_off, VTable vt, int root) {
+  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
+  const bool call_ok = sync_start(c, send_off, recv_off, s_a, s_b);
+  if (!call_ok) {
+    sync_end_failed(c);
+    return;
+  }
+  if (sizeof(U) == 1 || all_aligned_to(s_a, s_b, c.n, sizeof(U))) scatterv_pull_body<U, UNROLL>(c, s_a, s_b, vt, root);
+  else scatterv_pull_body<unsigned char, 1>(c, s_a, s_b, vt, root);
+  sync_end(c);
+}
+
+// ---------------------------------------------------------------------------------------------
 // Point-to-point and local copies: dst <- src, `bytes` bytes, any alignment.  src may be a peer
 // mapping (receiver pulls the sender's posted region over NVLink).
 // ---------------------------------------------------------------------------------------------

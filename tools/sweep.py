@@ -237,6 +237,55 @@ def main():
         send.free()
         recv.free()
 
+    rooted = [c for c in ("gather", "scatter", "allgatherv") if c in colls]
+    if rooted and n > 1:
+        # One algorithm each, blocking calls only: time = events around back-to-back calls, max over
+        # ranks.  Roofline: the busiest NVLink direction of any GPU (root's ingress for Gather, its
+        # egress for Scatter, for Allgatherv the larger of a rank's egress (n-1)*c_r and its
+        # ingress total-c_r) at 450 GB/s per direction (H100 SXM data sheet).
+        per_max = min(args.max_bytes // n, 128 << 20)
+        big = mpi.Alloc(per_max // 4 * n, np.float32)
+        small = mpi.Alloc(per_max // 4, np.float32).copy_from_host(np.full(per_max // 4, rank + 1, dtype=np.float32))
+        link = 450e9
+        for coll in rooted:
+            shapes = ("uniform", "skewed") if coll == "allgatherv" else ("uniform",)
+            for shape in shapes:
+                for S in [s for s in sizes if 4 * n <= s <= per_max]:
+                    cnt = S // 4  # elements per rank (uniform); skewed: rank n-1 carries half of n*cnt
+                    counts = [cnt] * n if shape == "uniform" else [cnt * n // (2 * (n - 1))] * (n - 1) + [cnt * n - cnt * n // (2 * (n - 1)) * (n - 1)]
+                    if max(counts) > per_max // 4:
+                        continue
+                    total = sum(counts)
+                    tab = (ctypes.c_size_t * n)(*counts)
+                    if coll == "gather":
+                        call = lambda: lib.b200mpi_gather(small.ptr, big.ptr, cnt, L.F32, 0, L.DEVICE)  # noqa: E731
+                        link_bytes = max(total - counts[0], max(counts))
+                    elif coll == "scatter":
+                        call = lambda: lib.b200mpi_scatter(big.ptr, small.ptr, cnt, L.F32, 0, L.DEVICE)  # noqa: E731
+                        link_bytes = max(total - counts[0], max(counts))
+                    else:
+                        call = lambda: lib.b200mpi_allgatherv(small.ptr, big.ptr, tab, L.F32, L.DEVICE)  # noqa: E731
+                        link_bytes = max(max(c * (n - 1), total - c) for c in counts)
+                    if coll == "scatter" and rank == 0:
+                        big[:total].copy_from_host(np.repeat(np.arange(1, n + 1, dtype=np.float32), cnt))
+                    it, wm = iters_for(total * 4)
+
+                    def blocking():
+                        if call():
+                            raise RuntimeError(L.last_error())
+                    t = timed(blocking, it, wm)
+                    ok = True  # checked where this rank's recv was written, up to 64 MiB
+                    if coll == "scatter":
+                        ok = cnt > (16 << 20) or bool(np.all(small[:cnt].to_host() == rank + 1))
+                    elif coll == "allgatherv" or rank == 0:
+                        ok = total > (16 << 20) or bool(np.array_equal(big[:total].to_host(), np.repeat(np.arange(1, n + 1, dtype=np.float32), counts)))
+                    ok = maxr(0.0 if ok else 1.0) == 0.0
+                    emit({"coll": coll, "dtype": "f32", "algo": shape, "root": 0 if coll != "allgatherv" else None, "counts": counts, "bytes": total * 4,
+                          "t_us": t * 1e6, "algbw_gbs": total * 4 / t / 1e9, "link_bytes": link_bytes * 4,
+                          "link_roofline_share": link_bytes * 4 / link / t, "ok": ok})
+        big.free()
+        small.free()
+
     if "p2p" in colls and n > 1:
         # bounce (examples/bounce/bounce.go:85-138): even sends, odd returns; device-resident float64
         maxp = min(args.max_bytes, 256 << 20)

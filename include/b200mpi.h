@@ -177,7 +177,7 @@ int b200mpi_get_algo(int coll, size_t count, int dtype); /* what AUTO resolves t
 int b200mpi_set_max_blocks(int blocks); /* cap grid size (0 = default: SMs x occupancy) */
 /* Tuning knobs for sweeps: "twoshot_unroll" (0|1), "nvls_unroll" (1|2|4|8), "nvls_min_ranks",
  * "nvls_max_blocks", "oneshot_max_bytes", "ll_max_bytes", "stage_chunk", "pipe_min_bytes",
- * "pipe_chunk_bytes", "bounce_chunk_bytes", "host_threads", "own_block_bytes", "copy_variant",
+ * "pipe_chunk_bytes", "bounce_chunk_bytes", "host_threads", "own_block_bytes",
  * "hybrid_p2p_permille", "hybrid_p2p_blocks", "hybrid_min_bytes", "bcast_nvls2", "bcast_nvls_min",
  * "allgather_nvls_min", "host_register" (pin pageable host slices in place, cached; 0 drops the cache),
  * "p2p_fast" (host-slice Send/Receive through mapped pinned buffers), "watchdog_ms". */

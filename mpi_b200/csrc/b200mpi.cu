@@ -154,7 +154,6 @@ struct Ctx {
   // pinned, device-mapped bounce buffers: a small host-slice Allreduce is a memcpy + ONE kernel that
   // reads its input over PCIe and writes result + completion word to host memory
   char* ll_host = nullptr; char* ll_dev = nullptr; // [in kLLCells*8][out kLLCells*8][done word]
-  int copy_variant = 5; // 16 vectors in flight per thread, 256 threads: best of 7 launch shapes on an H100 SXM (400 W limit), 1.42 TB/s algbw at 256 MiB, 1.43 at 1 GiB
   size_t hybrid_min_bytes = 32u << 20;
   int nvls_min_ranks = 4; // below this the fused two-shot moves fewer bytes per link than NVLS
   size_t own_block_bytes = 1u << 20; // interleave granularity of slice ownership (Owner in kernels.cuh)
@@ -336,28 +335,31 @@ static int launch_check(const char* what) {
   return 0;
 }
 
-// dst <- src on `s` with the library's own copy kernel (local HBM or peer mapping).
+// dst <- src on `s` with the library's own copy kernel (local HBM or peer mapping), any alignment:
+// 256 threads x 16 vectors in flight per thread, up to one CTA per SM (or max_blocks).
 static int launch_copy(void* dst, const void* src, size_t bytes, cudaStream_t s) {
   if (bytes == 0) return 0;
-  unsigned char* d = (unsigned char*)dst;
-  const unsigned char* c = (const unsigned char*)src;
-  const size_t nvec = (bytes + 15) / 16;
-  const int sms = g->sm_count;
-  auto grid = [&](int threads, int unroll, int per_sm) {
-    size_t want = (nvec + (size_t)threads * unroll - 1) / ((size_t)threads * unroll);
-    size_t cap = g->max_blocks > 0 ? (size_t)g->max_blocks : (size_t)sms * per_sm;
-    return (int)std::max<size_t>(1, std::min(want, cap));
-  };
-  switch (g->copy_variant) { // launch shapes for the HBM-bound local copy (bench.py --params copy_variant=N)
-    case 1: copy_bytes_kernel<8, 512, 1><<<grid(512, 8, 1), 512, 0, s>>>(d, c, bytes); break;
-    case 2: copy_bytes_kernel<4, 256, 2><<<grid(256, 4, 2), 256, 0, s>>>(d, c, bytes); break;
-    case 3: copy_bytes_kernel<8, 256, 2><<<grid(256, 8, 2), 256, 0, s>>>(d, c, bytes); break;
-    case 4: copy_bytes_kernel<4, 1024, 1><<<grid(1024, 4, 1), 1024, 0, s>>>(d, c, bytes); break;
-    case 5: copy_bytes_kernel<16, 256, 1><<<grid(256, 16, 1), 256, 0, s>>>(d, c, bytes); break;
-    case 7: copy_bytes_kernel<4, 512, 2><<<grid(512, 4, 2), 512, 0, s>>>(d, c, bytes); break;
-    default: copy_bytes_kernel<4, 512, 1><<<grid(512, 4, 1), 512, 0, s>>>(d, c, bytes); break;
-  }
+  constexpr size_t kPerBlock = 256 * 16 * 16; // bytes one CTA moves per grid pass
+  const size_t want = (bytes + kPerBlock - 1) / kPerBlock;
+  const size_t cap = g->max_blocks > 0 ? (size_t)g->max_blocks : (size_t)g->sm_count;
+  const int blocks = (int)std::max<size_t>(1, std::min(want, cap));
+  copy_bytes_kernel<16, 256, 1><<<blocks, 256, 0, s>>>((unsigned char*)dst, (const unsigned char*)src, bytes);
   return launch_check("copy_bytes_kernel");
+}
+
+// dst <- src where both ends are memory of this rank's GPU: copy_local_kernel with one thread per
+// 16-byte vector when src and dst agree mod 16 and the copy is at least kLocalCopyMinBytes (a grid
+// of up to 2^31 - 1 CTAs, or max_blocks), else launch_copy.  Below 8 MiB the grid-stride kernel was
+// as fast or faster on an H100 SXM (400 W): at 4 MiB 4.5 us against 6.7-7.9 us per call.
+static constexpr size_t kLocalCopyMinBytes = 8u << 20;
+static int launch_local_copy(void* dst, const void* src, size_t bytes, cudaStream_t s) {
+  if (bytes == 0) return 0;
+  if ((((uintptr_t)dst ^ (uintptr_t)src) & 15) || bytes < kLocalCopyMinBytes) return launch_copy(dst, src, bytes, s);
+  const size_t want = (bytes / 16 + kLocalCopyThreads - 1) / kLocalCopyThreads;
+  const size_t cap = g->max_blocks > 0 ? (size_t)g->max_blocks : (size_t)INT32_MAX;
+  const int blocks = (int)std::max<size_t>(1, std::min(want, cap));
+  copy_local_kernel<<<blocks, kLocalCopyThreads, 0, s>>>((unsigned char*)dst, (const unsigned char*)src, bytes);
+  return launch_check("copy_local_kernel");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -782,6 +784,21 @@ struct Buf {
   bool staged = false;
 };
 
+// True when [p, p + bytes) is memory of this rank's GPU: its own heap, or a buffer the runtime
+// reports as device memory on g->dev (not a peer's memory, not managed or host memory).
+static bool on_this_gpu(const void* p, size_t bytes) {
+  size_t off;
+  if (g->heap.contains(p, bytes, off)) return true;
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { (void)cudaGetLastError(); return false; }
+  return a.type == cudaMemoryTypeDevice && a.device == g->dev;
+}
+
+// Device-to-device copy between a caller's buffer `foreign` and a staging area in this rank's heap.
+static int stage_copy(void* dst, const void* src, size_t bytes, const void* foreign) {
+  return on_this_gpu(foreign, bytes) ? launch_local_copy(dst, src, bytes, g->stream) : launch_copy(dst, src, bytes, g->stream);
+}
+
 static int resolve_in(const void* p, size_t bytes, int memkind, int which, Buf& out) {
   size_t off;
   if (memkind == B200MPI_DEVICE && g->heap.contains(p, bytes, off)) {
@@ -796,7 +813,7 @@ static int resolve_in(const void* p, size_t bytes, int memkind, int which, Buf& 
   if (bytes) {
     char* dst = (char*)g->heap.base[g->ctrl.rank] + out.off;
     if (memkind == B200MPI_HOST) CUDA_OK(cudaMemcpyAsync(dst, p, bytes, cudaMemcpyHostToDevice, g->stream));
-    else { rc = launch_copy(dst, p, bytes, g->stream); if (rc) return rc; }
+    else { rc = stage_copy(dst, p, bytes, p); if (rc) return rc; }
   }
   return 0;
 }
@@ -819,7 +836,7 @@ static int copy_out(void* p, size_t bytes, int memkind, const Buf& b) {
   if (!b.staged || bytes == 0) return 0;
   const char* src = (const char*)g->heap.base[g->ctrl.rank] + b.off;
   if (memkind == B200MPI_HOST) CUDA_OK(cudaMemcpyAsync(p, src, bytes, cudaMemcpyDeviceToHost, g->stream));
-  else return launch_copy(p, src, bytes, g->stream);
+  else return stage_copy(p, src, bytes, p);
   return 0;
 }
 
@@ -839,7 +856,8 @@ static int local_copy(void* dst, const void* src, size_t bytes, int memkind, boo
     rc = copy_out(dst, bytes, memkind, b);
     if (rc) return rc;
   } else {
-    int rc = launch_copy(dst, src, bytes, g->stream);
+    const bool local = on_this_gpu(dst, bytes) && on_this_gpu(src, bytes);
+    int rc = local ? launch_local_copy(dst, src, bytes, g->stream) : launch_copy(dst, src, bytes, g->stream);
     if (rc) return rc;
   }
   return finish(async);
@@ -2112,7 +2130,6 @@ int b200mpi_set_param(const char* name, int64_t value) {
   if (k == "twoshot_unroll") g->twoshot_unroll = value ? 1 : 0;
   else if (k == "nvls_unroll") g->nvls_unroll = (int)value;
   else if (k == "nvls_min_ranks") g->nvls_min_ranks = (int)value;
-  else if (k == "copy_variant") g->copy_variant = (int)value;
   else if (k == "ll_max_bytes") g->ll_max_bytes = (size_t)std::min<int64_t>(std::max<int64_t>(value, 0), (int64_t)(ll_cells(g->ctrl.n) * 8));
   else if (k == "nvls_max_blocks") g->nvls_max_blocks = (int)std::max<int64_t>(1, value);
   else if (k == "oneshot_max_bytes") g->oneshot_max_bytes = (size_t)value;
@@ -2151,7 +2168,6 @@ int b200mpi_get_param(const char* name, int64_t* value) {
   else if (k == "nvls_unroll") *value = g->nvls_unroll;
   else if (k == "nvls_min_ranks") *value = g->nvls_min_ranks;
   else if (k == "nvls_max_blocks") *value = g->nvls_max_blocks;
-  else if (k == "copy_variant") *value = g->copy_variant;
   else if (k == "ll_max_bytes") *value = (int64_t)g->ll_max_bytes;
   else if (k == "oneshot_max_bytes") *value = (int64_t)g->oneshot_max_bytes;
   else if (k == "pipe_min_bytes") *value = (int64_t)g->pipe_min_bytes;

@@ -1560,6 +1560,32 @@ copy_bytes_kernel(unsigned char* __restrict__ dst, const unsigned char* __restri
 }
 
 // ---------------------------------------------------------------------------------------------
+// Local copy (both ends in this GPU's memory, (src ^ dst) & 15 == 0): one 16-byte vector per thread
+// and a grid that covers the whole message, so the block scheduler hands out CTAs as earlier ones
+// retire; there is no grid-stride loop whose last pass runs on a few SMs, and no per-thread burst of
+// loads followed by a burst of stores.  Threads 0..15 of CTA 0 also copy the < 16 head and tail
+// bytes outside the aligned span.  With a capped grid (b200mpi_set_max_blocks) the loop runs more
+// than once.
+// ---------------------------------------------------------------------------------------------
+constexpr int kLocalCopyThreads = 512;
+
+__global__ void __launch_bounds__(kLocalCopyThreads)
+copy_local_kernel(unsigned char* __restrict__ dst, const unsigned char* __restrict__ src, size_t bytes) {
+  size_t head = (16 - (reinterpret_cast<uintptr_t>(dst) & 15)) & 15;
+  if (head > bytes) head = bytes;
+  const size_t nvec = (bytes - head) / 16;
+  const uint4* __restrict__ s = reinterpret_cast<const uint4*>(src + head);
+  uint4* __restrict__ d = reinterpret_cast<uint4*>(dst + head);
+  const size_t stride = (size_t)gridDim.x * kLocalCopyThreads;
+  for (size_t i = (size_t)blockIdx.x * kLocalCopyThreads + threadIdx.x; i < nvec; i += stride) d[i] = s[i];
+  if (blockIdx.x == 0 && threadIdx.x < 16) {
+    const size_t t = threadIdx.x, tail0 = head + nvec * 16;
+    if (t < head) dst[t] = src[t];
+    if (tail0 + t < bytes) dst[tail0 + t] = src[tail0 + t];
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 // Allreduce, LL (low latency): bit-exact against the oracle in worlds of 2 and 4 ranks sharing one
 // H100 (tests/test_gpu_worlds.py::test_ll_...); its latency over NVLink has not been measured on
 // H100.  AUTO uses it on multi-GPU worlds up to "ll_max_bytes".

@@ -650,6 +650,53 @@ func (c *Cuda) Scatterv(send, recv interface{}, counts []int, root int) ([]int, 
 	return counts, nil
 }
 
+// Alltoallv: a nil recvCounts is learnt with one int64 Alltoall of sendCounts.
+func (c *Cuda) Alltoallv(send interface{}, sendCounts []int, recv interface{}, recvCounts []int) ([]int, error) {
+	sp, sn, sdt, sk, err := lowerTyped("Alltoallv", send)
+	if err != nil {
+		return nil, err
+	}
+	st, stotal, err := c.table("Alltoallv", sendCounts)
+	if err != nil {
+		return nil, err
+	}
+	if stotal != sn {
+		return nil, errors.New("mpi: Alltoallv send must hold sum(sendCounts) elements")
+	}
+	if recvCounts == nil {
+		mine, theirs := make([]int64, len(sendCounts)), make([]int64, len(sendCounts))
+		for i, v := range sendCounts {
+			mine[i] = int64(v)
+		}
+		if err := c.Alltoall(mine, theirs); err != nil {
+			return nil, err
+		}
+		recvCounts = make([]int, len(theirs))
+		for i, v := range theirs {
+			recvCounts[i] = int(v)
+		}
+	}
+	rt, rtotal, err := c.table("Alltoallv", recvCounts)
+	if err != nil {
+		return nil, err
+	}
+	r, err := resized("Alltoallv", recv, rtotal)
+	if err != nil {
+		return nil, err
+	}
+	rp, _, rdt, rk, err := lowerTyped("Alltoallv", r)
+	if err != nil {
+		return nil, err
+	}
+	if sdt != rdt || sk != rk {
+		return nil, errors.New("mpi: Alltoallv send and recv must have the same type and memory kind")
+	}
+	if rc := C.b200mpi_alltoallv(sp, &st[0], rp, &rt[0], sdt, sk); rc != 0 {
+		return nil, lastError(rc, 0)
+	}
+	return recvCounts, nil
+}
+
 func (c *Cuda) Barrier() error {
 	if rc := C.b200mpi_barrier(); rc != 0 {
 		return lastError(rc, 0)

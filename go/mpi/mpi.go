@@ -26,6 +26,7 @@
 //	ReduceScatter, Reduce, Alltoall   the usual MPI companions of the above
 //	Gather, Scatter                   rooted collection and distribution of equal blocks
 //	Gatherv, Scatterv, Allgatherv     the same with a different length on every rank
+//	Alltoallv                         Alltoall with a different length for every (source, destination) pair
 //	Isend + Wait   the non-blocking Send design the reference sketches and comments out (mpi.go:132-152)
 //
 // They are served through the optional Collective interface, the upgrade the reference hints at
@@ -80,6 +81,12 @@ type Collective3 interface {
 	Gatherv(send, recv interface{}, counts []int, root int) ([]int, error)
 	Scatterv(send, recv interface{}, counts []int, root int) ([]int, error)
 	Allgatherv(send, recv interface{}, counts []int) ([]int, error)
+}
+
+// Collective4 is the fourth optional upgrade: the variable-count exchange. Unlike Collective3's
+// tables, sendCounts and recvCounts are this rank's own row and column and differ from rank to rank.
+type Collective4 interface {
+	Alltoallv(send interface{}, sendCounts []int, recv interface{}, recvCounts []int) ([]int, error)
 }
 
 // Raw marks a payload that is sent as bytes without any encoding.
@@ -299,4 +306,16 @@ func Allgatherv(send, recv interface{}, counts []int) ([]int, error) {
 		return nil, err
 	}
 	return c.Allgatherv(send, recv, counts)
+}
+
+// Alltoallv sends block j of send (sendCounts[j] elements, packed in rank order) to rank j; the
+// block from rank r lands at offset recvCounts[0]+...+recvCounts[r-1] of recv, which is resized to
+// sum(recvCounts). recvCounts[r] must equal rank r's sendCounts[Rank()]; a nil recvCounts is learnt
+// with one Alltoall of sendCounts, and the table used is returned.
+func Alltoallv(send interface{}, sendCounts []int, recv interface{}, recvCounts []int) ([]int, error) {
+	c, ok := current.(Collective4)
+	if !ok {
+		return nil, fmt.Errorf("mpi: registered implementation %T has no Alltoallv", current)
+	}
+	return c.Alltoallv(send, sendCounts, recv, recvCounts)
 }

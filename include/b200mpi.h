@@ -31,7 +31,7 @@ extern "C" {
 #endif
 
 #define B200MPI_VERSION 200 /* 0.2.0: + isend/wait, reduce_scatter, reduce, alltoall, probes, get_param;
-                               then gather, scatter, gatherv, scatterv, allgatherv (all additive) */
+                               then gather, scatter, gatherv, scatterv, allgatherv, alltoallv (all additive) */
 #define B200MPI_MAX_RANKS 8 /* "the 8 GPUs of one box" */
 
 typedef enum {
@@ -161,6 +161,14 @@ int b200mpi_scatter(const void* send, void* recv, size_t count_per_rank, int dty
 int b200mpi_gatherv(const void* send, void* recv, const size_t* counts, int dtype, int root, int memkind);
 int b200mpi_scatterv(const void* send, void* recv, const size_t* counts, int dtype, int root, int memkind);
 int b200mpi_allgatherv(const void* send, void* recv, const size_t* counts, int dtype, int memkind);
+/* send holds sum(send_counts) elements: block j (send_counts[j] elements, packed in rank order)
+ * goes to rank j.  recv holds sum(recv_counts) elements: the block from rank r lands at
+ * recv_counts[0] + ... + recv_counts[r-1].  recv_counts[r] on rank j must equal send_counts[j] on
+ * rank r; ranks whose tables disagree get B200MPI_ERR_PEER, all of them, with no buffer touched.
+ * Any count may be 0.  send == recv (in place) is B200MPI_ERR_ARG, as for alltoall.  Buffers outside
+ * the b200mpi_alloc heap are staged whole through it (B200MPI_ERR_NOMEM if too big). */
+int b200mpi_alltoallv(const void* send, const size_t* send_counts, void* recv, const size_t* recv_counts,
+                      int dtype, int memkind);
 int b200mpi_barrier(void);
 
 /* Enqueue-only forms on the library stream (DEVICE memkind only). */

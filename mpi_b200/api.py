@@ -8,6 +8,7 @@ Same names, same argument meaning, same blocking behaviour:
     ReduceScatter(send, recv, op)  Reduce(send, recv, op, root)  Alltoall(send, recv)      (new)
     Gather(send, recv, root)  Scatter(send, recv, root)                                       (new)
     Gatherv(send, recv, root, counts)  Scatterv(send, recv, counts, root)  Allgatherv(send, recv, counts)
+    Alltoallv(send, send_counts, recv, recv_counts)                                          (new)
     Isend(data, destination, tag) + Wait(destination, tag)     (the Send/Wait design commented out
                                                                 in the reference, mpi.go:132-152)
 
@@ -435,6 +436,25 @@ class Cuda(Interface):
         _check(L.load().b200mpi_scatterv(sp, rp, table, rdt, int(root), rk))
         return recv, counts
 
+    def Alltoallv(self, send, send_counts, recv=None, recv_counts=None):
+        """Block j of send (send_counts[j] elements, packed in rank order) goes to rank j; the block
+        from rank r lands at displacement recv_counts[0]+...+recv_counts[r-1] of recv.  recv_counts[r]
+        must equal rank r's send_counts[Rank()]; omitted, it is learnt with one int64 Alltoall of
+        send_counts.  A host recv is created or resized as in Gatherv.  Returns (recv, recv_counts)."""
+        rank, n = self._world()
+        sp, sc, sdt, sk, keep, _ = _describe(send)
+        send_counts, stable = self._table(send_counts, n)
+        if sum(send_counts) != sc:
+            raise ValueError("mpi: Alltoallv send must hold sum(send_counts) elements")
+        if recv_counts is None:
+            learnt = np.empty(n, dtype=np.int64)
+            self.Alltoall(np.array(send_counts, dtype=np.int64), learnt)
+            recv_counts = learnt.tolist()
+        recv_counts, rtable = self._table(recv_counts, n)
+        recv, rp = self._recv_for(recv, sum(recv_counts), sdt, sk, "Alltoallv")
+        _check(L.load().b200mpi_alltoallv(sp, stable, rp, rtable, sdt, sk))
+        return recv, recv_counts
+
 
 # ---- package-level facade: mpi.go:56-159 -------------------------------------------------------
 _mpier = Cuda()
@@ -536,6 +556,10 @@ def Scatterv(send, recv, counts=None, root=0):
 
 def Allgatherv(send, recv=None, counts=None):
     return _collective("Allgatherv")(send, recv, counts)
+
+
+def Alltoallv(send, send_counts, recv=None, recv_counts=None):
+    return _collective("Alltoallv")(send, send_counts, recv, recv_counts)
 
 
 def Isend(data, destination, tag):

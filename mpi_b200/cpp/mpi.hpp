@@ -14,7 +14,7 @@
 //   mpi.Register(impl)                         void mpi::Register(Interface*)  (second call throws = panics, mpi.go:61-67)
 //   flag.Parse() + mpi.Flag*                   mpi::ParseFlags(argc, argv) + mpi::Flag*
 //   new: Recv, Bcast, Allreduce, Allgather, Barrier, ReduceScatter, Reduce, Alltoall, Isend/Wait,
-//        Gather, Scatter, Gatherv, Scatterv, Allgatherv;
+//        Gather, Scatter, Gatherv, Scatterv, Allgatherv, Alltoallv;
 //        mpi::DeviceSlice<T> for heap-resident buffers
 // `data` may be std::vector<double|float|int64_t|uint8_t>, std::string (sent as bytes, the
 // "anything else is gob-encoded" path), or DeviceSlice<T>.
@@ -181,6 +181,8 @@ struct Interface {
   virtual Error Gatherv(Buffer, Buffer, const size_t*, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Gatherv"; return e; }
   virtual Error Scatterv(Buffer, Buffer, const size_t*, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Scatterv"; return e; }
   virtual Error Allgatherv(Buffer, Buffer, const size_t*) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Allgatherv"; return e; }
+  // send_counts / recv_counts[Size()]: this rank's row and column of the exchange (they differ from rank to rank)
+  virtual Error Alltoallv(Buffer, const size_t*, Buffer, const size_t*) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Alltoallv"; return e; }
   // the Send/Wait pair the reference sketches and comments out (mpi.go:132-152)
   virtual Error Isend(Buffer, int, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Isend"; return e; }
   virtual Error Wait(int, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Wait"; return e; }
@@ -220,6 +222,7 @@ struct Cuda : Interface {
   Error Gatherv(Buffer s, Buffer r, const size_t* counts, int root) override { return make_error(b200mpi_gatherv(s.ptr, r.ptr, counts, s.dtype, root, s.memkind)); }
   Error Scatterv(Buffer s, Buffer r, const size_t* counts, int root) override { return make_error(b200mpi_scatterv(s.ptr, r.ptr, counts, r.dtype, root, r.memkind)); }
   Error Allgatherv(Buffer s, Buffer r, const size_t* counts) override { return make_error(b200mpi_allgatherv(s.ptr, r.ptr, counts, s.dtype, s.memkind)); }
+  Error Alltoallv(Buffer s, const size_t* sc, Buffer r, const size_t* rc) override { return make_error(b200mpi_alltoallv(s.ptr, sc, r.ptr, rc, s.dtype, s.memkind)); }
   Error Isend(Buffer d, int destination, int tag) override { return make_error(b200mpi_isend(d.ptr, d.count, d.dtype, destination, tag, d.memkind)); }
   Error Wait(int destination, int tag) override { return make_error(b200mpi_wait(destination, tag)); }
 };
@@ -359,6 +362,25 @@ template <typename T> inline Error Scatterv(const std::vector<T>& send, std::vec
     recv->resize((*counts)[(size_t)Rank()]);
   }
   return mpier()->Scatterv(lower(send), lower(*recv), counts->data(), root);
+}
+
+// Alltoallv: block j of send (send_counts[j] elements, packed in rank order) goes to rank j.  An empty
+// *recv_counts is learnt through one int64 Alltoall of send_counts; *recv is resized to
+// sum(*recv_counts), as Receive resizes.
+template <typename T> inline Error Alltoallv(const std::vector<T>& send, const std::vector<size_t>& send_counts, std::vector<T>* recv,
+                                             std::vector<size_t>* recv_counts) {
+  const size_t n = (size_t)(Size() > 0 ? Size() : 0);
+  if (n > 0 && send_counts.size() != n) return arg_error("mpi: Alltoallv send_counts must hold Size() entries");
+  if (n > 0 && sum_of(send_counts) != send.size()) return arg_error("mpi: Alltoallv send must hold sum(send_counts) elements");
+  if (n > 0 && recv_counts->empty()) {
+    std::vector<int64_t> mine(send_counts.begin(), send_counts.end()), theirs;
+    Error e = Alltoall(mine, &theirs);
+    if (e) return e;
+    recv_counts->assign(theirs.begin(), theirs.end());
+  }
+  if (n > 0 && recv_counts->size() != n) return arg_error("mpi: Alltoallv recv_counts must hold Size() entries");
+  recv->resize(sum_of(*recv_counts));
+  return mpier()->Alltoallv(lower(send), send_counts.data(), lower(*recv), recv_counts->data());
 }
 
 template <typename D> inline Error Isend(const D& data, int destination, int tag) { return mpier()->Isend(lower(data), destination, tag); }

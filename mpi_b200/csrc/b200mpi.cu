@@ -258,7 +258,6 @@ static int grid_for(size_t units_per_rank, int unroll) {
 
 // Every launch advances the epoch by kEpochStride whatever the algorithm (kernels.cuh), so ranks
 // that disagreed about one call still agree about the flag values of the next.
-static uint64_t mix64(uint64_t x);
 static Comm next_comm() {
   // Every kScrubEvery-th launch (the same one on every rank: epochs move in lockstep) is preceded by
   // scrub_kernel, which rewrites every slot row so that no flag word can fall 2^31 behind the epoch.
@@ -312,14 +311,11 @@ static int check_status() {
 
 // What this rank thinks the call is, folded into one word; equal on every rank of a well-formed
 // call.  coll: 0 allreduce, 1 bcast, 2 allgather, 3 barrier, 4 reduce_scatter, 5 reduce, 6 alltoall,
-// 7 gather(v), 8 scatter(v), 9 allgatherv (these three carry a hash of the counts table in `total`).
+// 7 gather(v), 8 scatter(v), 9 allgatherv (these three carry a hash of the counts table in `total`),
+// 10 alltoallv (whose ranks hold different tables: each adds its table digest to the signature it
+// announces, see sync_start_pairs in kernels.cuh).
 // `total` is the element count of the whole user call when the launch is one chunk of a pipelined
 // host-slice call (ranks that disagree about the total then disagree from the first chunk on).
-static uint64_t mix64(uint64_t x) {
-  x ^= x >> 30; x *= 0xbf58476d1ce4e5b9ull;
-  x ^= x >> 27; x *= 0x94d049bb133111ebull;
-  return x ^ (x >> 31);
-}
 static uint64_t make_sig(int coll, int dtype, int extra, int algo, size_t count, size_t total = 0) {
   uint64_t h = mix64((uint64_t)count + 0x9e3779b97f4a7c15ull);
   h = mix64(h ^ ((uint64_t)(coll & 15) << 40 | (uint64_t)(dtype & 15) << 32 | (uint64_t)(extra & 0xffff) << 16 | (uint64_t)(algo & 0xffff)));
@@ -1396,6 +1392,61 @@ static int do_gather(const void* send, void* recv, size_t count, int dtype, int 
   return scatter ? do_scatterv(send, recv, counts.data(), dtype, root, memkind) : do_gatherv(send, recv, counts.data(), dtype, root, false, memkind);
 }
 
+// Alltoallv.  The grid is block_cap() CTAs whatever the table: the barriers pair CTAs by blockIdx and
+// the grid is part of the signature, so it may depend only on what every rank shares.  The access
+// unit follows this rank's offsets and both of its displacement tables; a peer whose offsets are less
+// aligned sends this rank to the byte-wide body (kernels.cuh).
+template <typename U>
+static void launch_alltoallv_u(Comm& c, uint64_t a, uint64_t b, const VTable& sv, const VTable& rv, uint64_t digest, cudaStream_t s) {
+  constexpr int UNROLL = 4;
+  const int blocks = block_cap();
+  sig_grid(c, blocks);
+  const uint64_t base_sig = c.sig;
+  c.sig = base_sig + digest;
+  alltoallv_push_kernel<U, UNROLL><<<blocks, kThreads, 0, s>>>(c, a, b, sv, rv, base_sig);
+}
+static int launch_alltoallv(uint64_t a, uint64_t b, const VTable& sv, const VTable& rv, uint64_t digest, cudaStream_t s) {
+  Comm c = next_comm();
+  uint64_t m = a | b;
+  for (int r = 0; r <= c.n; ++r) m |= sv.off[r] | rv.off[r];
+  if ((m & 15) == 0) launch_alltoallv_u<uint4>(c, a, b, sv, rv, digest, s);
+  else if ((m & 7) == 0) launch_alltoallv_u<unsigned long long>(c, a, b, sv, rv, digest, s);
+  else if ((m & 3) == 0) launch_alltoallv_u<unsigned int>(c, a, b, sv, rv, digest, s);
+  else launch_alltoallv_u<unsigned char>(c, a, b, sv, rv, digest, s);
+  return launch_check("alltoallv_push_kernel");
+}
+
+// Alltoallv: block j of send (send_counts[j] elements, packed in rank order) goes to rank j, where it
+// lands at displacement recv_counts[0] + ... + recv_counts[rank()-1] of that rank's recv.  Every rank
+// holds a different table, so the tables are checked on the device (sync_start_pairs) and a
+// mismatch ends as B200MPI_ERR_PEER on every rank with no buffer touched.
+static int do_alltoallv(const void* send, const size_t* send_counts, void* recv, const size_t* recv_counts, int dtype, int memkind) {
+  int rc = need_data_plane();
+  if (rc) return rc;
+  const int n = g->ctrl.n, me = g->ctrl.rank;
+  size_t es;
+  if ((rc = check_v_args("alltoallv", dtype, memkind, es))) return rc;
+  if (!send_counts || !recv_counts) return fail(B200MPI_ERR_ARG, "alltoallv: NULL counts table");
+  VTable sv, rv;
+  uint64_t digest;
+  if (!a2av_tables(me, n, send_counts, recv_counts, es, sv, rv, digest)) return fail(B200MPI_ERR_ARG, "alltoallv: sum(counts) * element size overflows");
+  const size_t sbytes = sv.off[n], rbytes = rv.off[n];
+  if ((sbytes && !send) || (rbytes && !recv)) return fail(B200MPI_ERR_ARG, "alltoallv: NULL buffer with count > 0");
+  if (send == recv && (sbytes || rbytes)) return fail(B200MPI_ERR_ARG, "alltoallv: in place is not supported");
+  if (n == 1) {
+    if (send_counts[0] != recv_counts[0]) return fail(B200MPI_ERR_PEER, "alltoallv: send_counts[0] != recv_counts[0] in a world of one; buffers were left untouched");
+    return local_copy(recv, send, sbytes, memkind, false);
+  }
+  Buf in, out;
+  if ((rc = resolve_in(send, sbytes, memkind, 0, in))) return rc;
+  if ((rc = resolve_out(recv, rbytes, memkind, 1, out))) return rc;
+  g->cur_sig = make_sig(10, dtype, 0, 0, 0);
+  rc = launch_alltoallv(in.off, out.off, sv, rv, digest, g->stream);
+  if (rc) return rc;
+  if ((rc = copy_out_checked(recv, rbytes, memkind, out))) return rc;
+  return finish(false);
+}
+
 // ---------------------------------------------------------------------------------------------
 // point to point
 // ---------------------------------------------------------------------------------------------
@@ -2079,6 +2130,9 @@ int b200mpi_scatter(const void* send, void* recv, size_t count_per_rank, int dty
 int b200mpi_gatherv(const void* send, void* recv, const size_t* counts, int dtype, int root, int memkind) { return do_gatherv(send, recv, counts, dtype, root, false, memkind); }
 int b200mpi_scatterv(const void* send, void* recv, const size_t* counts, int dtype, int root, int memkind) { return do_scatterv(send, recv, counts, dtype, root, memkind); }
 int b200mpi_allgatherv(const void* send, void* recv, const size_t* counts, int dtype, int memkind) { return do_gatherv(send, recv, counts, dtype, 0, true, memkind); }
+int b200mpi_alltoallv(const void* send, const size_t* send_counts, void* recv, const size_t* recv_counts, int dtype, int memkind) {
+  return do_alltoallv(send, send_counts, recv, recv_counts, dtype, memkind);
+}
 int b200mpi_reduce_scatter_async(const void* send, void* recv, size_t count_per_rank, int dtype, int op) { return do_reduce_scatter(send, recv, count_per_rank, dtype, op, B200MPI_DEVICE, true); }
 int b200mpi_bcast_async(void* buf, size_t count, int dtype, int root) { return do_bcast(buf, count, dtype, root, B200MPI_DEVICE, true); }
 int b200mpi_allreduce_async(const void* send, void* recv, size_t count, int dtype, int op) { return do_allreduce(send, recv, count, dtype, op, B200MPI_DEVICE, true); }

@@ -67,6 +67,14 @@ struct Comm {
   uint64_t sig;              // what this rank thinks the call is: (count, collective, dtype, op, algorithm)
 };
 
+// The splitmix64 finaliser, a bijection of 64-bit words: folds call signatures (b200mpi.cu:
+// make_sig) and the Alltoallv table digest (a2av_tables).
+__host__ __device__ inline uint64_t mix64(uint64_t x) {
+  x ^= x >> 30; x *= 0xbf58476d1ce4e5b9ull;
+  x ^= x >> 27; x *= 0x94d049bb133111ebull;
+  return x ^ (x >> 31);
+}
+
 // ---------------------------------------------------------------------------------------------
 // flag primitives
 // ---------------------------------------------------------------------------------------------
@@ -200,6 +208,61 @@ __device__ __forceinline__ bool sync_start(const Comm& c, uint64_t a, uint64_t b
   const int v = *verdict;
   if (v) {
     if (t == 0 && v != 3) { // a watchdog expiry has already raised status 1
+      *(volatile uint32_t*)c.status = 2u;
+      __threadfence_system();
+    }
+    return false;
+  }
+  return true;
+}
+
+// The start barrier of a call whose ranks hold different tables (Alltoallv).  Thread t announces
+// values meant for rank t alone: a_t = the bytes this rank expects from t, b_t = the heap offset where
+// t's block lands here.  On return s_a[t] = the bytes t expects from this rank, s_b[t] = where this
+// rank's block lands in t's heap.  The signatures differ from rank to rank (c.sig = base_sig + this
+// rank's table digest): the call is well formed when the n announced words sum to n * base_sig.
+// Every rank sums the same n words (each rank writes one signature into every slot row), so every
+// rank reaches the same verdict -- over row 0 first for CTAs other than 0, as sync_start does, then
+// over its own row.  Each pair also compares its byte counts exactly (s_a[t] against want_t), so even
+// a digest collision could not let this rank write more than a peer expects.  Verdicts and exits are
+// sync_start's, and sync_end / sync_end_failed follow as usual.
+__device__ __forceinline__ bool sync_start_pairs(const Comm& c, uint64_t base_sig, uint64_t a_t, uint64_t b_t, uint64_t want_t,
+                                                 uint64_t* s_a, uint64_t* s_b) {
+  __shared__ unsigned long long sums[2]; // of row 0, of this CTA's row (mod 2^64)
+  int* verdict = start_verdict();
+  const int t = threadIdx.x;
+  const unsigned long long want_sum = (unsigned long long)c.n * base_sig;
+  if (t == 0) { *verdict = 0; sums[0] = 0; sums[1] = 0; }
+  __syncthreads();
+  uint64_t pa, pb, psig;
+  if (t < c.n) {
+    Slot* theirs = slot_of(c, t, blockIdx.x, c.rank);
+    st_cell16(&theirs->cell[0], make_uint4((uint32_t)a_t, c.epoch, (uint32_t)(a_t >> 32), c.epoch));
+    st_cell16(&theirs->cell[1], make_uint4((uint32_t)b_t, c.epoch, (uint32_t)(b_t >> 32), c.epoch));
+    st_cell16(&theirs->cell[2], make_uint4((uint32_t)c.sig, c.epoch, (uint32_t)(c.sig >> 32), c.epoch));
+    if (blockIdx.x != 0) {
+      if (!wait_cells(slot_of(c, c.rank, 0, t), c.epoch, c, pa, pb, psig)) atomicMax(verdict, 3);
+      else atomicAdd(&sums[0], (unsigned long long)psig);
+    }
+  }
+  __syncthreads();
+  if (t == 0 && blockIdx.x != 0 && *verdict == 0 && sums[0] != want_sum) *verdict = 2;
+  __syncthreads();
+  if (t < c.n && *verdict == 0) {
+    if (!wait_cells(slot_of(c, c.rank, blockIdx.x, t), c.epoch, c, pa, pb, psig)) atomicMax(verdict, 3);
+    else {
+      s_a[t] = pa;
+      s_b[t] = pb;
+      atomicAdd(&sums[1], (unsigned long long)psig);
+      if (pa != want_t) atomicMax(verdict, 1);
+    }
+  }
+  __syncthreads();
+  if (t == 0 && *verdict == 0 && sums[1] != want_sum) *verdict = 1;
+  __syncthreads();
+  const int v = *verdict;
+  if (v) {
+    if (t == 0 && v != 3) {
       *(volatile uint32_t*)c.status = 2u;
       __threadfence_system();
     }
@@ -1519,6 +1582,99 @@ scatterv_pull_kernel(Comm c, uint64_t send_off, uint64_t recv_off, VTable vt, in
   }
   if (sizeof(U) == 1 || all_aligned_to(s_a, s_b, c.n, sizeof(U))) scatterv_pull_body<U, UNROLL>(c, s_a, s_b, vt, root);
   else scatterv_pull_body<unsigned char, 1>(c, s_a, s_b, vt, root);
+  sync_end(c);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Alltoallv: rank i holds its send row S_i[0..n) and its recv column R_i[0..n) of an n x n matrix of
+// block sizes; the call is consistent when R_j[i] == S_i[j] for every pair.  The tables differ from
+// rank to rank, so they cannot be hashed into one shared signature.  Instead rank i announces
+// base_sig + D_i with the zero-sum digest
+//     D_i = sum_j f(i, j, S_i[j] bytes) - sum_k f(k, i, R_i[k] bytes)   (mod 2^64),
+// where every consistent entry appears once with + (at its sender) and once with - (at its
+// receiver), so the D_i of a consistent matrix sum to 0 (sync_start_pairs).  For fixed (src, dst),
+// f is a bijection of the byte count (xor with a per-pair key, then the splitmix64 finaliser), so a
+// change of any single entry always changes the sum; other changes (a swap of two entries) escape
+// only by a 64-bit collision, and even then the per-pair byte check keeps every store in bounds.
+// ---------------------------------------------------------------------------------------------
+__host__ __device__ inline uint64_t a2av_term(int src, int dst, uint64_t bytes) {
+  return mix64(bytes ^ mix64(0x616c6c746f616c6cull + (uint64_t)(src * kMaxRanks + dst)));
+}
+
+// Rank `me`'s byte displacements (send: of the block for rank j; recv: of the block from rank k; off[n]
+// = total, off[r] = total for r > n) and its digest D_me.  false when a count times the element size,
+// or a sum of them, does not fit in 64 bits.
+__host__ __device__ inline bool a2av_tables(int me, int n, const size_t* send_counts, const size_t* recv_counts, size_t es,
+                                            VTable& sv, VTable& rv, uint64_t& digest) {
+  uint64_t so = 0, ro = 0, d = 0;
+  for (int r = 0; r < n; ++r) {
+    sv.off[r] = so;
+    rv.off[r] = ro;
+    if (send_counts[r] > (UINT64_MAX - so) / es || recv_counts[r] > (UINT64_MAX - ro) / es) return false;
+    so += send_counts[r] * es;
+    ro += recv_counts[r] * es;
+    d += a2av_term(me, r, send_counts[r] * es) - a2av_term(r, me, recv_counts[r] * es);
+  }
+  for (int r = n; r <= kMaxRanks; ++r) {
+    sv.off[r] = so;
+    rv.off[r] = ro;
+  }
+  digest = d;
+  return true;
+}
+
+// Push: every rank reads its n send blocks once from local HBM and stores block j at s_b[j] of rank
+// j's heap, targets rotated with the own block last (a local copy).  Each target's range is
+// grid-strided over all CTAs, so a skewed table still spreads over the whole grid.  s_src[j] is the
+// heap offset of block j in this rank's send, s_len[j] its bytes.
+template <typename U, int UNROLL>
+__device__ __forceinline__ void alltoallv_push_body(const Comm& c, const uint64_t* s_src, const uint64_t* s_len, const uint64_t* s_b) {
+  const int n = c.n;
+  const size_t step = (size_t)gridDim.x * blockDim.x * UNROLL;
+  for (int k = 0; k < n; ++k) {
+    const int j = (c.rank + 1 + k) % n;
+    const size_t units = s_len[j] / sizeof(U);
+    const U* src = reinterpret_cast<const U*>(c.base[c.rank] + s_src[j]);
+    U* dst = reinterpret_cast<U*>(c.base[j] + s_b[j]);
+    for (size_t i0 = (size_t)blockIdx.x * blockDim.x * UNROLL + threadIdx.x; i0 < units; i0 += step) {
+      U v[UNROLL];
+#pragma unroll
+      for (int u = 0; u < UNROLL; ++u) {
+        const size_t i = i0 + (size_t)u * blockDim.x;
+        if (i < units) v[u] = src[i];
+      }
+#pragma unroll
+      for (int u = 0; u < UNROLL; ++u) {
+        const size_t i = i0 + (size_t)u * blockDim.x;
+        if (i < units) dst[i] = v[u];
+      }
+    }
+  }
+}
+
+// sv / rv: this rank's send and recv displacements (a2av_tables); c.sig = base_sig + its digest.
+// U was picked by the host from this rank's offsets and displacements; a peer whose destination
+// offsets are less aligned sends this rank to the byte-wide body.
+template <typename U, int UNROLL>
+__global__ void __launch_bounds__(kThreads, 1)
+alltoallv_push_kernel(Comm c, uint64_t send_off, uint64_t recv_off, VTable sv, VTable rv, uint64_t base_sig) {
+  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks], s_src[kMaxRanks];
+  const int t = threadIdx.x;
+  uint64_t slo = 0, shi = 0, rlo = 0, rhi = 0;
+  if (t < c.n) {
+    vtable_range(sv, t, slo, shi);
+    vtable_range(rv, t, rlo, rhi);
+    s_src[t] = send_off + slo;
+  }
+  const bool call_ok = sync_start_pairs(c, base_sig, rhi - rlo, recv_off + rlo, shi - slo, s_a, s_b);
+  if (!call_ok) {
+    sync_end_failed(c);
+    return;
+  }
+  uint64_t m = 0;
+  for (int r = 0; r < c.n; ++r) m |= s_b[r];
+  if (sizeof(U) == 1 || (m & (sizeof(U) - 1)) == 0) alltoallv_push_body<U, UNROLL>(c, s_src, s_a, s_b);
+  else alltoallv_push_body<unsigned char, 1>(c, s_src, s_a, s_b);
   sync_end(c);
 }
 

@@ -286,6 +286,49 @@ def main():
         big.free()
         small.free()
 
+    exchange = [c for c in ("alltoall", "alltoallv") if c in colls]
+    if exchange and n > 1:
+        # S = bytes of every rank's send.  Alltoallv runs a uniform table and a skewed one (half of
+        # every rank's send to its right neighbour, the rest evenly to the others).  Roofline per GPU:
+        # the larger of its egress sum_{j!=i} S_i[j] and its ingress sum_{k!=i} R_i[k], the busiest GPU
+        # over 450 GB/s per direction (H100 SXM data sheet).  Block (i -> j) holds i*n + j + 1.
+        per_max = min(args.max_bytes, 512 << 20)
+        sbuf = mpi.Alloc(per_max // 4, np.float32)
+        rbuf = mpi.Alloc(per_max // 4, np.float32)
+        link = 450e9
+        for coll in exchange:
+            shapes = ("uniform", "skewed") if coll == "alltoallv" else ("uniform",)
+            for shape in shapes:
+                for S in [s for s in sizes if 4 * n <= s <= per_max // 2]:
+                    cnt = S // 4 // n
+                    if shape == "uniform":
+                        m = [[cnt] * n for _ in range(n)]
+                    else:
+                        half, rest = cnt * n // 2, (cnt * n - cnt * n // 2) // (n - 1)
+                        m = [[half if j == (i + 1) % n else rest for j in range(n)] for i in range(n)]
+                    scounts, rcounts = m[rank], [m[k][rank] for k in range(n)]
+                    sbuf[:sum(scounts)].copy_from_host(np.repeat(np.arange(rank * n + 1, rank * n + n + 1, dtype=np.float32), scounts))
+                    stab, rtab = (ctypes.c_size_t * n)(*scounts), (ctypes.c_size_t * n)(*rcounts)
+                    if coll == "alltoall":
+                        call = lambda: lib.b200mpi_alltoall(sbuf.ptr, rbuf.ptr, cnt, L.F32, L.DEVICE)  # noqa: E731
+                    else:
+                        call = lambda: lib.b200mpi_alltoallv(sbuf.ptr, stab, rbuf.ptr, rtab, L.F32, L.DEVICE)  # noqa: E731
+                    link_bytes = max(max(sum(m[i]) - m[i][i], sum(m[k][i] for k in range(n)) - m[i][i]) for i in range(n))
+                    it, wm = iters_for(S)
+
+                    def blocking():
+                        if call():
+                            raise RuntimeError(L.last_error())
+                    t = timed(blocking, it, wm)
+                    want = np.repeat(np.arange(n, dtype=np.float32) * n + rank + 1, rcounts)
+                    ok = sum(rcounts) * 4 > (64 << 20) or bool(np.array_equal(rbuf[:sum(rcounts)].to_host(), want))
+                    ok = maxr(0.0 if ok else 1.0) == 0.0
+                    emit({"coll": coll, "dtype": "f32", "algo": shape, "counts": scounts, "bytes": sum(scounts) * 4,
+                          "t_us": t * 1e6, "algbw_gbs": sum(scounts) * 4 / t / 1e9, "link_bytes": link_bytes * 4,
+                          "link_roofline_share": link_bytes * 4 / link / t, "ok": ok})
+        sbuf.free()
+        rbuf.free()
+
     if "p2p" in colls and n > 1:
         # bounce (examples/bounce/bounce.go:85-138): even sends, odd returns; device-resident float64
         maxp = min(args.max_bytes, 256 << 20)

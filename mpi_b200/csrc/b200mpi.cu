@@ -150,7 +150,8 @@ struct Ctx {
   int nvls_unroll = 2;      // multi-GPU switch tuning: not yet measured on H100 (tools/sweep.py re-derives it)
   int nvls_max_blocks = 48; // fewer requests in flight suit the switch reduction; not yet measured on H100
   size_t ll_max_bytes = 0; // AUTO uses the barrier-free LL allreduce for messages up to this size (<= 256 KiB)
-  uint32_t ll_seq = 0;
+  uint32_t ll_seq = 0;          // the last LL sequence number issued (ll_seq_next, kernels.cuh)
+  bool ll_wrap_pending = false; // a resync crossed 2^32: the next LL call clears the lanes first
   // pinned, device-mapped bounce buffers: a small host-slice Allreduce is a memcpy + ONE kernel that
   // reads its input over PCIe and writes result + completion word to host memory
   char* ll_host = nullptr; char* ll_dev = nullptr; // [in kLLCells*8][out kLLCells*8][done word]
@@ -284,18 +285,23 @@ static Comm next_comm() {
 // rank), so every rank comes here.
 static void resync_after_error(bool peers_alive) {
   if (g->ctrl.n == 1) return;
-  struct { uint32_t epoch, ll_seq; } mine = {g->epoch, g->ll_seq}, all[B200MPI_MAX_RANKS];
+  struct { uint32_t epoch, ll_seq, ll_wrap_pending; } mine = {g->epoch, g->ll_seq, g->ll_wrap_pending ? 1u : 0u}, all[B200MPI_MAX_RANKS];
   std::string err;
   // A mismatched call ends on every rank, so everybody comes here and the exchange is prompt.  After
   // a watchdog expiry a peer may be gone or stuck: do not trade one hang for another.
   const int64_t wait_ns = peers_alive ? 30ll * 1000000000ll : 2ll * 1000000000ll;
   if (g->ctrl.allgather(&mine, sizeof mine, all, err, wait_ns) != 0) return; // nothing to agree with
   for (int r = 0; r < g->ctrl.n; ++r) {
-    if ((int32_t)(all[r].epoch - g->epoch) > 0) g->epoch = all[r].epoch;
-    if ((int32_t)(all[r].ll_seq - g->ll_seq) > 0) g->ll_seq = all[r].ll_seq;
+    if (!flag_reached(g->epoch, all[r].epoch)) g->epoch = all[r].epoch;
+    if (!flag_reached(g->ll_seq, all[r].ll_seq)) g->ll_seq = all[r].ll_seq;
+    if (all[r].ll_wrap_pending) g->ll_wrap_pending = true;
   }
   g->epoch += kEpochStride;
-  g->ll_seq += 2; // keep the parity, skip cells a failed call may have half written
+  // keep the parity, skip cells a failed call may have half written; when this crosses 2^32 the next
+  // LL call clears the lanes first
+  const LLSeqNext next = ll_seq_next(g->ll_seq, 2);
+  g->ll_seq = next.seq;
+  if (next.wrapped) g->ll_wrap_pending = true;
 }
 
 static int check_status() {
@@ -859,11 +865,40 @@ static int local_copy(void* dst, const void* src, size_t bytes, int memkind, boo
   return finish(async);
 }
 
+// A device-wide rendezvous with nothing in between, on `s`.
+static int launch_barrier(cudaStream_t s) {
+  g->cur_sig = make_sig(3, 0, 0, 0, 0);
+  Comm c = next_comm();
+  sig_grid(c, 1);
+  barrier_kernel<<<1, 32, 0, s>>>(c);
+  return launch_check("barrier_kernel");
+}
+
+// The LL sequence has crossed 2^32 (ll_seq_next): a lane cell may already hold the value about to be
+// issued, zeros from Init or a value written 2^32 calls ago.  A barrier (no peer is still pushing cells
+// of an earlier call), this rank's lanes of both parities cleared, a second barrier (no peer pushes
+// its next cells before they are clear).  ll_seq agrees on every rank, so every rank comes here on
+// the same call, once per 2^32 LL calls.
+static int clear_ll_lanes(cudaStream_t s) {
+  int rc = launch_barrier(s);
+  if (rc) return rc;
+  CUDA_OK(cudaMemsetAsync((char*)g->heap.base[g->ctrl.rank] + kLLOff, 0, kLLRegionCells * sizeof(uint4), s));
+  rc = launch_barrier(s);
+  if (rc) return rc;
+  g->ll_wrap_pending = false;
+  return 0;
+}
+
 // Barrier-free LL allreduce for small messages (kernels.cuh): any local device pointers.
 template <typename T, typename Op>
 static int launch_ll_t(const void* send, void* recv, size_t count, uint32_t* done_host, cudaStream_t s) {
   Comm c = g->comm;
-  const uint32_t seq = ++g->ll_seq;
+  const LLSeqNext next = ll_seq_next(g->ll_seq, 1);
+  if (next.wrapped || g->ll_wrap_pending) {
+    const int rc = clear_ll_lanes(s);
+    if (rc) return rc;
+  }
+  const uint32_t seq = g->ll_seq = next.seq;
   const size_t ncell = (count * sizeof(T) + 7) / 8;
   const int blocks = (int)std::max<size_t>(1, std::min<size_t>((ncell + 255) / 256, 128)); // one cell per thread up to 256 KiB
   allreduce_ll_kernel<T, Op><<<blocks, 256, 0, s>>>(c, (const T*)send, (T*)recv, count, seq, done_host);
@@ -900,6 +935,8 @@ static int allreduce_ll_host(const void* send, void* recv, size_t count, int dty
   CUDA_OK(cudaStreamSynchronize(g->stream)); // enqueue-only calls issued earlier may still be running
   if (bytes) memcpy(g->ll_host, send, bytes);
   volatile uint32_t* done = (volatile uint32_t*)(g->ll_host + 2 * half);
+  *done = 0; // no sequence number is 0: the word cannot match before this call's kernel writes it
+             // (after a restart of the sequence it may still hold this call's value from 2^32 calls ago)
   int rc = launch_ll(dtype, op, g->ll_dev, g->ll_dev + half, count, (uint32_t*)(g->ll_dev + 2 * half), g->stream);
   if (rc) return rc;
   const uint32_t seq = g->ll_seq;
@@ -1812,6 +1849,27 @@ static void apply_defaults() {
   if (const char* w = getenv("B200MPI_HYBRID_PERMILLE")) g->hybrid_p2p_permille = std::max(0, std::min(900, atoi(w)));
 }
 
+// Test hook (B200MPI_EPOCH_START = e): give this rank's control region the state of a long-running job
+// about to launch epoch e instead of zeros.  Every slot cell holds the oldest value a scrubbed row may
+// hold, every slot flag e - 1, every ring step counter the value of one launch earlier.  The LL lanes
+// stay zero, as a job's lanes beyond its largest message are.  Peers first write into this heap after
+// Init's final barrier, so the preset needs no synchronisation.
+static int preset_control_region(uint32_t e) {
+  std::vector<Slot> slots((size_t)kMaxBlocks * kMaxRanks);
+  const uint32_t oldest = e - kScrubEvery * kEpochStride;
+  for (Slot& s : slots) {
+    memset(&s, 0, sizeof s);
+    for (uint4& cell : s.cell) cell = make_uint4(0, oldest, 0, oldest);
+    s.flag = e - 1;
+  }
+  const std::vector<uint32_t> ring(kMaxBlocks, (e - kEpochStride) * 8u);
+  char* base = (char*)g->heap.base[g->ctrl.rank];
+  CUDA_OK(cudaMemcpy(base, slots.data(), slots.size() * sizeof(Slot), cudaMemcpyHostToDevice));
+  CUDA_OK(cudaMemcpy(base + kRingFlagsOff, ring.data(), ring.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+  CUDA_OK(cudaDeviceSynchronize());
+  return 0;
+}
+
 int b200mpi_init(const char* addr, const char* alladdr_csv, const char* password, int64_t timeout_ns, int gpu) {
   std::lock_guard<std::mutex> lock(g_mu);
   if (g && g->initialised) return fail(B200MPI_ERR_ARG, "mpi: Init called twice");
@@ -1858,23 +1916,37 @@ int b200mpi_init(const char* addr, const char* alladdr_csv, const char* password
   if (prop.major != 9 || prop.minor != 0) return bail(B200MPI_ERR_NO_DEVICE, std::string("device '") + prop.name + "' is not sm_90 (H100-class); this library ships sm_90a code only");
   if (!g->drv.load(err)) return bail(B200MPI_ERR_CUDA, err);
   if (!(getenv("B200MPI_NUMA") && atoi(getenv("B200MPI_NUMA")) == 0)) g->gpu_numa_node = numa_node_of_gpu(g->dev);
-  if (const char* w = getenv("B200MPI_SCRUB_EVERY")) {
-    uint32_t v = (uint32_t)std::max(2, atoi(w)), p2 = 2;
-    while (p2 * 2 <= v) p2 *= 2;
-    g->scrub_every = p2;
-  }
+  CounterEnv cenv;
+  const std::string cenv_err = parse_counter_env(getenv("B200MPI_SCRUB_EVERY"), getenv("B200MPI_EPOCH_START"), getenv("B200MPI_LL_SEQ_START"),
+                                                 kScrubEvery, kEpochStride, cenv);
+  g->scrub_every = cenv.scrub_every;
+  g->epoch = cenv.epoch_start;
+  g->ll_seq = cenv.ll_seq_start;
   if (const char* w = getenv("B200MPI_HOST_THREADS")) g->host_threads = std::max(0, atoi(w));
   if (const char* w = getenv("B200MPI_HOST_REGISTER")) g->host_register = atoi(w) != 0;
 
-  // who sits where: ranks sharing a device (functional-test mode) rule out NVLS
-  struct Hello { unsigned char uuid[16]; int32_t dev; int32_t mc; } mine = {}, all[B200MPI_MAX_RANKS];
+  // who sits where: ranks sharing a device (functional-test mode) rule out NVLS.  The counter settings
+  // travel along: ranks that disagree on them (or a rank that could not parse them) fail Init on every
+  // rank instead of hanging in the first collective.
+  struct Hello { unsigned char uuid[16]; int32_t dev; int32_t mc; uint32_t epoch_start, ll_seq_start, env_ok; } mine = {}, all[B200MPI_MAX_RANKS];
   memcpy(mine.uuid, &prop.uuid, 16);
   mine.dev = g->dev;
   int mc = 0;
   g->drv.DeviceGetAttribute(&mc, CU_DEVICE_ATTRIBUTE_MULTICAST_SUPPORTED, g->dev);
   mine.mc = mc;
+  mine.epoch_start = cenv.epoch_start;
+  mine.ll_seq_start = cenv.ll_seq_start;
+  mine.env_ok = cenv_err.empty() ? 1u : 0u;
   rc = g->ctrl.allgather(&mine, sizeof mine, all, err);
   if (rc) return bail(rc, err);
+  if (!cenv_err.empty()) return bail(B200MPI_ERR_ARG, cenv_err);
+  for (int a = 0; a < g->ctrl.n; ++a) {
+    if (!all[a].env_ok) return bail(B200MPI_ERR_ARG, "rank " + std::to_string(a) + " rejected its B200MPI_SCRUB_EVERY / B200MPI_EPOCH_START / B200MPI_LL_SEQ_START");
+    if (all[a].epoch_start != mine.epoch_start || all[a].ll_seq_start != mine.ll_seq_start)
+      return bail(B200MPI_ERR_ARG, "ranks disagree on B200MPI_EPOCH_START / B200MPI_LL_SEQ_START: rank " + std::to_string(a) + " has " +
+                                       std::to_string(all[a].epoch_start) + " / " + std::to_string(all[a].ll_seq_start) + ", this rank " +
+                                       std::to_string(mine.epoch_start) + " / " + std::to_string(mine.ll_seq_start));
+  }
   bool want_nvls = g->ctrl.n > 1;
   if (const char* w = getenv("B200MPI_NVLS")) want_nvls = want_nvls && atoi(w) != 0;
   for (int a = 0; a < g->ctrl.n; ++a) {
@@ -1925,6 +1997,7 @@ int b200mpi_init(const char* addr, const char* alladdr_csv, const char* password
   g->comm.rank = g->ctrl.rank;
   g->comm.n = g->ctrl.n;
   apply_defaults();
+  if (cenv.preset && preset_control_region(cenv.epoch_start)) return bail(B200MPI_ERR_CUDA, t_err);
   rc = g->ctrl.barrier(err);
   if (rc) return bail(rc, err);
   g->initialised = true;
@@ -2153,11 +2226,7 @@ int b200mpi_barrier(void) {
     return rc ? fail(rc, err) : 0;
   }
   if (g->ctrl.n == 1) return finish(false);
-  g->cur_sig = make_sig(3, 0, 0, 0, 0);
-  Comm c = next_comm();
-  sig_grid(c, 1);
-  barrier_kernel<<<1, 32, 0, g->stream>>>(c);
-  int rc = launch_check("barrier_kernel");
+  int rc = launch_barrier(g->stream);
   if (rc) return rc;
   return finish(false);
 }
@@ -2240,6 +2309,8 @@ int b200mpi_get_param(const char* name, int64_t* value) {
   else if (k == "allgather_nvls_min") *value = (int64_t)g->allgather_nvls_min;
   else if (k == "sm_count") *value = g->sm_count;
   else if (k == "shared_device") *value = g->shared_device ? 1 : 0;
+  else if (k == "epoch") *value = (int64_t)g->epoch;
+  else if (k == "ll_seq") *value = (int64_t)g->ll_seq;
   else return fail(B200MPI_ERR_ARG, "get_param: unknown parameter '" + k + "'");
   return 0;
 }

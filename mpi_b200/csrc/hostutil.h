@@ -1,7 +1,9 @@
 // hostutil.h -- host-only helpers of libb200mpi (no CUDA in this file, so they are unit-tested and
 // run under ThreadSanitizer on a CPU box: tests/cpp/hostutil_test.cpp).
 #pragma once
+#include <errno.h>
 #include <sched.h>
+#include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -152,5 +154,57 @@ struct CopyPool {
     threads.clear();
   }
 };
+
+// ---------------------------------------------------------------------------------------------
+// Counter settings read at Init.
+//   B200MPI_SCRUB_EVERY   launches between two flag scrubs: a power of two (rounded down, at least 2),
+//                         clamped to max_scrub.  It can only lower the period: a longer one would let a
+//                         flag word fall 2^31 behind and look "ahead".
+//   B200MPI_EPOCH_START   (test hook) epoch of the first launch; must be 1 mod `stride`, the only values
+//                         the launch schedule produces.
+//   B200MPI_LL_SEQ_START  (test hook) the LL sequence number held after Init.
+// Values are decimal.  A null string leaves the default.  Returns "" or what is wrong (Init then fails with B200MPI_ERR_ARG).
+// ---------------------------------------------------------------------------------------------
+struct CounterEnv {
+  uint32_t scrub_every;
+  uint32_t epoch_start = 1;
+  uint32_t ll_seq_start = 0;
+  bool preset = false; // B200MPI_EPOCH_START was given: preset the control region for that epoch
+};
+// Plain decimal digits only (no sign, blanks or base prefixes), at most 2^32 - 1.
+static inline bool parse_u32(const char* s, uint32_t& v) {
+  if (!s || !*s) return false;
+  uint64_t x = 0;
+  for (const char* p = s; *p; ++p) {
+    if (*p < '0' || *p > '9') return false;
+    x = x * 10 + (uint64_t)(*p - '0');
+    if (x > 0xffffffffull) return false;
+  }
+  v = (uint32_t)x;
+  return true;
+}
+static inline std::string parse_counter_env(const char* scrub, const char* epoch, const char* ll_seq, uint32_t max_scrub,
+                                            uint32_t stride, CounterEnv& out) {
+  out = CounterEnv();
+  out.scrub_every = max_scrub;
+  uint32_t v = 0;
+  if (scrub) {
+    if (!parse_u32(scrub, v)) return std::string("B200MPI_SCRUB_EVERY is not a decimal integer: '") + scrub + "'";
+    uint32_t p2 = 2;
+    while (p2 < max_scrub && p2 * 2 <= v) p2 *= 2;
+    out.scrub_every = std::min(p2, max_scrub);
+  }
+  if (epoch) {
+    if (!parse_u32(epoch, v)) return std::string("B200MPI_EPOCH_START is not a 32-bit decimal integer: '") + epoch + "'";
+    if (v % stride != 1) return "B200MPI_EPOCH_START must be 1 mod " + std::to_string(stride) + ", got " + std::to_string(v);
+    out.epoch_start = v;
+    out.preset = true;
+  }
+  if (ll_seq) {
+    if (!parse_u32(ll_seq, v)) return std::string("B200MPI_LL_SEQ_START is not a 32-bit decimal integer: '") + ll_seq + "'";
+    out.ll_seq_start = v;
+  }
+  return "";
+}
 
 } // namespace b200

@@ -75,6 +75,33 @@ __host__ __device__ inline uint64_t mix64(uint64_t x) {
   return x ^ (x >> 31);
 }
 
+// The wrap-safe comparison of every barrier: flag word `v` has reached `want` when it is at most
+// 2^31 - 1 ahead of it.  Sound only while no word lags the value it is compared with by 2^31 or
+// more (scrub_kernel keeps it so).
+__host__ __device__ __forceinline__ bool flag_reached(uint32_t v, uint32_t want) { return (int32_t)(v - want) >= 0; }
+// flag_reached for six words at once.  A difference v - want has its sign bit set exactly when
+// flag_reached(v, want) is false, so all six have reached `want` when the OR of their differences
+// has a clear sign bit: six subtractions, three ORs and one sign test per poll, as the start
+// barrier's spin compiled to when it was written out by hand.  (A chain of six flag_reached calls,
+// with & or &&, compiles to longer code.)
+__host__ __device__ __forceinline__ bool flags_reached(uint32_t v0, uint32_t v1, uint32_t v2, uint32_t v3, uint32_t v4, uint32_t v5, uint32_t want) {
+  return flag_reached(want + ((v0 - want) | (v1 - want) | (v2 - want) | (v3 - want) | (v4 - want) | (v5 - want)), want);
+}
+
+// LL sequence numbers (allreduce_ll_kernel).  A peer's cell counts as arrived when both its flag
+// words equal the call's sequence number, so a value must never meet a cell written 2^32 values
+// earlier, nor the zeros of a cleared lane.  The next value after `last` when `step` are consumed
+// (1 for an LL call, 2 for resync_after_error, which skips one value of each parity): never 0, and
+// `wrapped` is set when the advance crosses 2^32.  The sequence then restarts at 1, and the caller
+// must clear the LL lanes of every rank before the next LL kernel runs.
+struct LLSeqNext { uint32_t seq; bool wrapped; };
+__host__ __device__ inline LLSeqNext ll_seq_next(uint32_t last, uint32_t step) {
+  const uint32_t v = last + step;
+  if (v < last) return {1u, true}; // also covers landing on 0 exactly
+
+  return {v, false};
+}
+
 // ---------------------------------------------------------------------------------------------
 // flag primitives
 // ---------------------------------------------------------------------------------------------
@@ -105,7 +132,7 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
 __device__ __forceinline__ bool wait_flag(const uint32_t* p, uint32_t want, const Comm& c) {
   unsigned long long t0 = 0;
   uint32_t it = 0;
-  while ((int32_t)(ld_acquire_sys(p) - want) < 0) {
+  while (!flag_reached(ld_acquire_sys(p), want)) {
     if ((++it & 0xfffu) == 0) {
       unsigned long long now = globaltimer_ns();
       if (t0 == 0) t0 = now;
@@ -151,8 +178,7 @@ __device__ __forceinline__ bool wait_cells(const Slot* s, uint32_t epoch, const 
     // >= (wrap-safe), not ==: in normal operation a peer is never ahead (it waits for this CTA at its end
     // barrier), so the two are the same; after a failed call a peer may already be announcing its next
     // one, and a late CTA must then see "newer, different signature" at once instead of spinning.
-    if ((int32_t)(x.y - epoch) >= 0 && (int32_t)(x.w - epoch) >= 0 && (int32_t)(y.y - epoch) >= 0 && (int32_t)(y.w - epoch) >= 0 &&
-        (int32_t)(z.y - epoch) >= 0 && (int32_t)(z.w - epoch) >= 0) {
+    if (flags_reached(x.y, x.w, y.y, y.w, z.y, z.w, epoch)) {
       a = ((uint64_t)x.z << 32) | x.x;
       b = ((uint64_t)y.z << 32) | y.x;
       sig = ((uint64_t)z.z << 32) | z.x;

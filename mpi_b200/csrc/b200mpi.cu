@@ -536,65 +536,67 @@ static int launch_allreduce_hybrid_t(uint64_t so, uint64_t ro, size_t count, cud
   return launch_check("allreduce_hybrid_kernel");
 }
 
+// The reductions the kernels are instantiated for: f32, f64 and i64 with sum, max and min.  Returns
+// f(T{}, Op{}) for (dtype, op), or otherwise() for any other pair.
+template <typename T, typename F, typename G>
+static auto with_op(int op, F& f, G& otherwise) {
+  switch (op) {
+    case B200MPI_SUM: return f(T{}, OpSum{});
+    case B200MPI_MAX: return f(T{}, OpMax{});
+    case B200MPI_MIN: return f(T{}, OpMin{});
+  }
+  return otherwise();
+}
+template <typename F, typename G>
+static auto with_reduction(int dtype, int op, F&& f, G&& otherwise) {
+  switch (dtype) {
+    case B200MPI_F32: return with_op<float>(op, f, otherwise);
+    case B200MPI_F64: return with_op<double>(op, f, otherwise);
+    case B200MPI_I64: return with_op<long long>(op, f, otherwise);
+  }
+  return otherwise();
+}
+
+// The reductions the switch performs in multimem.ld_reduce: sums of f32, f64 and i64, min/max of
+// i64 only.  The NVLS kernels are instantiated for exactly these.
+template <typename T, typename Op>
+static constexpr bool switch_reduces() { return std::is_same<Op, OpSum>::value || std::is_same<T, long long>::value; }
+
 static bool nvls_supports(int dtype, int op) {
-  if (op == B200MPI_SUM) return dtype == B200MPI_F32 || dtype == B200MPI_F64 || dtype == B200MPI_I64;
-  return dtype == B200MPI_I64; // min/max: integer only in the switch
+  return with_reduction(dtype, op, [](auto t, auto o) { return switch_reduces<decltype(t), decltype(o)>(); }, [] { return false; });
 }
 
 // `total`: element count of the whole user call when this launch is one chunk of it, else 0.
 static int launch_allreduce(int algo, int dtype, int op, uint64_t so, uint64_t ro, size_t count, cudaStream_t s, size_t total = 0) {
   g->cur_sig = make_sig(0, dtype, op, algo, count, total);
-  if (algo == B200MPI_ALGO_NVLS || algo == B200MPI_ALGO_HYBRID) {
-    const bool hyb = algo == B200MPI_ALGO_HYBRID;
-#define B200_NVLS(T, OP) return hyb ? launch_allreduce_hybrid_t<T, OP>(so, ro, count, s) : launch_allreduce_nvls_t<T, OP>(so, ro, count, -1, s);
-    if (dtype == B200MPI_F32 && op == B200MPI_SUM) { B200_NVLS(float, OpSum) }
-    if (dtype == B200MPI_F64 && op == B200MPI_SUM) { B200_NVLS(double, OpSum) }
-    if (dtype == B200MPI_I64 && op == B200MPI_SUM) { B200_NVLS(long long, OpSum) }
-    if (dtype == B200MPI_I64 && op == B200MPI_MAX) { B200_NVLS(long long, OpMax) }
-    if (dtype == B200MPI_I64 && op == B200MPI_MIN) { B200_NVLS(long long, OpMin) }
-#undef B200_NVLS
-    return fail(B200MPI_ERR_UNSUPPORTED, "allreduce: NVLS supports sum (f32,f64,i64) and min/max (i64) only");
-  }
-#define B200_DISPATCH(T)                                                                         \
-  switch (op) {                                                                                  \
-    case B200MPI_SUM: return launch_allreduce_t<T, OpSum>(algo, so, ro, count, s);            \
-    case B200MPI_MAX: return launch_allreduce_t<T, OpMax>(algo, so, ro, count, s);            \
-    case B200MPI_MIN: return launch_allreduce_t<T, OpMin>(algo, so, ro, count, s);            \
-  }                                                                                              \
-  break;
-  switch (dtype) {
-    case B200MPI_F32: B200_DISPATCH(float)
-    case B200MPI_F64: B200_DISPATCH(double)
-    case B200MPI_I64: B200_DISPATCH(long long)
-  }
-#undef B200_DISPATCH
-  return fail(B200MPI_ERR_UNSUPPORTED, "allreduce: unsupported dtype/op (need f32, f64 or i64 with sum/max/min)");
+  const bool nvls = algo == B200MPI_ALGO_NVLS || algo == B200MPI_ALGO_HYBRID;
+  const char* nvls_only = "allreduce: NVLS supports sum (f32,f64,i64) and min/max (i64) only";
+  return with_reduction(
+      dtype, op,
+      [&](auto t, auto o) {
+        using T = decltype(t);
+        using Op = decltype(o);
+        if (!nvls) return launch_allreduce_t<T, Op>(algo, so, ro, count, s);
+        if constexpr (switch_reduces<T, Op>())
+          return algo == B200MPI_ALGO_HYBRID ? launch_allreduce_hybrid_t<T, Op>(so, ro, count, s) : launch_allreduce_nvls_t<T, Op>(so, ro, count, -1, s);
+        else return fail(B200MPI_ERR_UNSUPPORTED, nvls_only);
+      },
+      [&] { return fail(B200MPI_ERR_UNSUPPORTED, nvls ? nvls_only : "allreduce: unsupported dtype/op (need f32, f64 or i64 with sum/max/min)"); });
 }
 
 // Reduce to `root`: the owner-reduces bodies with a single destination.
 static int launch_reduce(int algo, int dtype, int op, uint64_t so, uint64_t ro, size_t count, int root, cudaStream_t s) {
   g->cur_sig = make_sig(5, dtype, op | (root << 4), algo, count);
-  if (algo == B200MPI_ALGO_NVLS) {
-    if (dtype == B200MPI_F32 && op == B200MPI_SUM) return launch_allreduce_nvls_t<float, OpSum>(so, ro, count, root, s);
-    if (dtype == B200MPI_F64 && op == B200MPI_SUM) return launch_allreduce_nvls_t<double, OpSum>(so, ro, count, root, s);
-    if (dtype == B200MPI_I64 && op == B200MPI_SUM) return launch_allreduce_nvls_t<long long, OpSum>(so, ro, count, root, s);
-    if (dtype == B200MPI_I64 && op == B200MPI_MAX) return launch_allreduce_nvls_t<long long, OpMax>(so, ro, count, root, s);
-    if (dtype == B200MPI_I64 && op == B200MPI_MIN) return launch_allreduce_nvls_t<long long, OpMin>(so, ro, count, root, s);
-  }
-#define B200_DISPATCH(T)                                                                                          \
-  switch (op) {                                                                                                   \
-    case B200MPI_SUM: return launch_allreduce_body_t<T, OpSum>(B200MPI_ALGO_TWOSHOT, so, ro, count, root, s);   \
-    case B200MPI_MAX: return launch_allreduce_body_t<T, OpMax>(B200MPI_ALGO_TWOSHOT, so, ro, count, root, s);   \
-    case B200MPI_MIN: return launch_allreduce_body_t<T, OpMin>(B200MPI_ALGO_TWOSHOT, so, ro, count, root, s);   \
-  }                                                                                                               \
-  break;
-  switch (dtype) {
-    case B200MPI_F32: B200_DISPATCH(float)
-    case B200MPI_F64: B200_DISPATCH(double)
-    case B200MPI_I64: B200_DISPATCH(long long)
-  }
-#undef B200_DISPATCH
-  return fail(B200MPI_ERR_UNSUPPORTED, "reduce: unsupported dtype/op (need f32, f64 or i64 with sum/max/min)");
+  return with_reduction(
+      dtype, op,
+      [&](auto t, auto o) {
+        using T = decltype(t);
+        using Op = decltype(o);
+        if (algo != B200MPI_ALGO_NVLS) return launch_allreduce_body_t<T, Op>(B200MPI_ALGO_TWOSHOT, so, ro, count, root, s);
+        if constexpr (switch_reduces<T, Op>()) return launch_allreduce_nvls_t<T, Op>(so, ro, count, root, s);
+        else return fail(B200MPI_ERR_UNSUPPORTED, "reduce: NVLS supports sum (f32,f64,i64) and min/max (i64) only");
+      },
+      [] { return fail(B200MPI_ERR_UNSUPPORTED, "reduce: unsupported dtype/op (need f32, f64 or i64 with sum/max/min)"); });
 }
 
 template <typename T, typename Op>
@@ -616,25 +618,22 @@ static int launch_reduce_scatter_nvls_t(uint64_t so, uint64_t ro, size_t count, 
   return launch_check("reduce_scatter_nvls_kernel");
 }
 
-template <typename T>
-static int launch_reduce_scatter_op(bool nvls, int op, uint64_t so, uint64_t ro, size_t count, cudaStream_t s) {
-  switch (op) {
-    case B200MPI_SUM: return nvls ? launch_reduce_scatter_nvls_t<T>(so, ro, count, s) : launch_reduce_scatter_p2p_t<T, OpSum>(so, ro, count, s);
-    case B200MPI_MAX: return launch_reduce_scatter_p2p_t<T, OpMax>(so, ro, count, s);
-    case B200MPI_MIN: return launch_reduce_scatter_p2p_t<T, OpMin>(so, ro, count, s);
-  }
-  return fail(B200MPI_ERR_ARG, "reduce_scatter: unknown op");
-}
-
 static int launch_reduce_scatter(int algo, int dtype, int op, uint64_t so, uint64_t ro, size_t count, cudaStream_t s) {
   const bool nvls = algo == B200MPI_ALGO_NVLS && op == B200MPI_SUM; // the switch form is instantiated for sums
   g->cur_sig = make_sig(4, dtype, op, nvls ? B200MPI_ALGO_NVLS : B200MPI_ALGO_TWOSHOT, count);
-  switch (dtype) {
-    case B200MPI_F32: return launch_reduce_scatter_op<float>(nvls, op, so, ro, count, s);
-    case B200MPI_F64: return launch_reduce_scatter_op<double>(nvls, op, so, ro, count, s);
-    case B200MPI_I64: return launch_reduce_scatter_op<long long>(nvls, op, so, ro, count, s);
-  }
-  return fail(B200MPI_ERR_UNSUPPORTED, "reduce_scatter: dtype must be f32, f64 or i64");
+  return with_reduction(
+      dtype, op,
+      [&](auto t, auto o) {
+        using T = decltype(t);
+        using Op = decltype(o);
+        if constexpr (std::is_same<Op, OpSum>::value)
+          if (nvls) return launch_reduce_scatter_nvls_t<T>(so, ro, count, s);
+        return launch_reduce_scatter_p2p_t<T, Op>(so, ro, count, s);
+      },
+      [&] {
+        const bool known_dtype = dtype == B200MPI_F32 || dtype == B200MPI_F64 || dtype == B200MPI_I64;
+        return known_dtype ? fail(B200MPI_ERR_ARG, "reduce_scatter: unknown op") : fail(B200MPI_ERR_UNSUPPORTED, "reduce_scatter: dtype must be f32, f64 or i64");
+      });
 }
 
 // AUTO for Allreduce: best busbw / latency per (n, size) among the variants.  The multi-GPU thresholds
@@ -700,40 +699,26 @@ static int pick_reduce_scatter(size_t, int dtype, int op) {
   return can && g->ctrl.n >= g->nvls_min_ranks ? B200MPI_ALGO_NVLS : B200MPI_ALGO_TWOSHOT;
 }
 
-// which: 0 allgather push, 1 allgather ring, 2 bcast (extra = root, mode 0 one-shot / 1 two-shot), 3 alltoall
-// The grid is a function of the byte count only: ranks may instantiate different access widths
-// (their offsets differ in alignment) but must launch the same number of CTAs, because the
-// barriers pair CTAs by blockIdx.
-template <typename U>
-static void launch_units_u(int which, Comm& c, uint64_t a, uint64_t b, size_t bytes, int extra, int mode, cudaStream_t s) {
-  constexpr int UNROLL = 4;
-  const size_t vecs = bytes / 16 + 1;
-  const size_t work = (which == 2 && mode == 1) ? vecs / (size_t)(c.n - 1) + 1 : vecs;
-  const int blocks = grid_for(work, UNROLL);
-  sig_grid(c, blocks);
-  if (which == 0) allgather_push_kernel<U, UNROLL><<<blocks, kThreads, 0, s>>>(c, a, b, bytes);
-  else if (which == 1) allgather_ring_kernel<U><<<blocks, kThreads, 0, s>>>(c, a, b, bytes);
-  else if (which == 3) alltoall_kernel<U, UNROLL><<<blocks, kThreads, 0, s>>>(c, a, b, bytes);
-  else bcast_kernel<U, UNROLL><<<blocks, kThreads, 0, s>>>(c, a, bytes, extra, mode);
-}
-static int launch_units(int which, Comm& c, uint64_t a, uint64_t b, size_t bytes, int extra, int mode, cudaStream_t s) {
-  // The widest access unit that divides the size and THIS rank's offsets.  Peers may be aligned
-  // differently: after sync_start every rank knows all offsets and drops to the byte-wide body if
-  // some peer's are narrower than its own unit (kernels.cuh: all_aligned_to).
-  const uint64_t m = a | b | bytes;
-  if ((m & 15) == 0) launch_units_u<uint4>(which, c, a, b, bytes, extra, mode, s);
-  else if ((m & 7) == 0) launch_units_u<unsigned long long>(which, c, a, b, bytes, extra, mode, s);
-  else if ((m & 3) == 0) launch_units_u<unsigned int>(which, c, a, b, bytes, extra, mode, s);
-  else launch_units_u<unsigned char>(which, c, a, b, bytes, extra, mode, s);
-  return launch_check(which == 2 ? "bcast_kernel" : which == 3 ? "alltoall_kernel" : "allgather kernel");
+// Calls f(U{}) with the widest access unit U (uint4, 8, 4 or 1 byte) dividing m, the OR of THIS
+// rank's offsets, sizes and displacements.  Peers may be aligned differently: after the start
+// barrier every rank knows all offsets and drops to the byte-wide body if some peer's are narrower
+// than its own unit (kernels.cuh: all_aligned_to).  Ranks may so instantiate different units but
+// must launch the same number of CTAs, because the barriers pair CTAs by blockIdx: a grid never
+// depends on U.
+template <typename F>
+static void with_unit(uint64_t m, F&& f) {
+  if ((m & 15) == 0) f(uint4{});
+  else if ((m & 7) == 0) f(0ull);
+  else if ((m & 3) == 0) f(0u);
+  else f((unsigned char)0);
 }
 
 // Bcast of `bytes` at heap offset `off` on every... (each rank passes its own offset)
 static int launch_bcast(int algo, int dtype, size_t count, uint64_t off, size_t bytes, int root, cudaStream_t s, size_t total = 0) {
   g->cur_sig = make_sig(1, dtype, root, algo, count, total);
   Comm c = next_comm();
+  const size_t nvec = bytes / 16 + 1;
   if (algo == B200MPI_ALGO_NVLS) {
-    const size_t nvec = bytes / 16 + 1;
     if (g->bcast_nvls2) {
       const size_t per = (nvec + c.n - 1) / c.n;
       const int blocks = grid_for(per, 4);
@@ -746,19 +731,28 @@ static int launch_bcast(int algo, int dtype, size_t count, uint64_t off, size_t 
     bcast_nvls_kernel<4><<<blocks, kThreads, 0, s>>>(c, off, bytes, root);
     return launch_check("bcast_nvls_kernel");
   }
-  return launch_units(2, c, off, off, bytes, root, algo == B200MPI_ALGO_TWOSHOT ? 1 : 0, s);
+  const int mode = algo == B200MPI_ALGO_TWOSHOT ? 1 : 0; // two-shot: each non-root moves one slice
+  const int blocks = grid_for(mode ? nvec / (size_t)(c.n - 1) + 1 : nvec, 4);
+  sig_grid(c, blocks);
+  with_unit(off | bytes, [&](auto u) { bcast_kernel<decltype(u), 4><<<blocks, kThreads, 0, s>>>(c, off, bytes, root, mode); });
+  return launch_check("bcast_kernel");
 }
 
 static int launch_allgather(int algo, int dtype, size_t count, uint64_t in_off, uint64_t out_off, size_t bytes, cudaStream_t s, size_t total = 0) {
   g->cur_sig = make_sig(2, dtype, 0, algo, count, total);
   Comm c = next_comm();
+  const int blocks = grid_for(bytes / 16 + 1, 4);
+  sig_grid(c, blocks);
   if (algo == B200MPI_ALGO_NVLS) {
-    const int blocks = grid_for(bytes / 16 + 1, 4);
-    sig_grid(c, blocks);
     allgather_nvls_kernel<4><<<blocks, kThreads, 0, s>>>(c, in_off, out_off, bytes);
     return launch_check("allgather_nvls_kernel");
   }
-  return launch_units(algo == B200MPI_ALGO_RING ? 1 : 0, c, in_off, out_off, bytes, 0, 0, s);
+  with_unit(in_off | out_off | bytes, [&](auto u) {
+    using U = decltype(u);
+    if (algo == B200MPI_ALGO_RING) allgather_ring_kernel<U><<<blocks, kThreads, 0, s>>>(c, in_off, out_off, bytes);
+    else allgather_push_kernel<U, 4><<<blocks, kThreads, 0, s>>>(c, in_off, out_off, bytes);
+  });
+  return launch_check("allgather kernel");
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -905,20 +899,9 @@ static int launch_ll_t(const void* send, void* recv, size_t count, uint32_t* don
   return launch_check("allreduce_ll_kernel");
 }
 static int launch_ll(int dtype, int op, const void* send, void* recv, size_t count, uint32_t* done_host, cudaStream_t s) {
-#define B200_LL(T)                                                                       \
-  switch (op) {                                                                          \
-    case B200MPI_SUM: return launch_ll_t<T, OpSum>(send, recv, count, done_host, s);     \
-    case B200MPI_MAX: return launch_ll_t<T, OpMax>(send, recv, count, done_host, s);     \
-    case B200MPI_MIN: return launch_ll_t<T, OpMin>(send, recv, count, done_host, s);     \
-  }                                                                                      \
-  break;
-  switch (dtype) {
-    case B200MPI_F32: B200_LL(float)
-    case B200MPI_F64: B200_LL(double)
-    case B200MPI_I64: B200_LL(long long)
-  }
-#undef B200_LL
-  return fail(B200MPI_ERR_UNSUPPORTED, "allreduce(LL): unsupported dtype/op");
+  return with_reduction(
+      dtype, op, [&](auto t, auto o) { return launch_ll_t<decltype(t), decltype(o)>(send, recv, count, done_host, s); },
+      [] { return fail(B200MPI_ERR_UNSUPPORTED, "allreduce(LL): unsupported dtype/op"); });
 }
 
 // Small host-slice Allreduce: memcpy into a device-mapped pinned buffer, ONE kernel that loads its
@@ -1286,7 +1269,10 @@ static int do_alltoall(const void* send, void* recv, size_t count, int dtype, in
   if (rc) return rc;
   g->cur_sig = make_sig(6, dtype, 0, 0, count);
   Comm c = next_comm();
-  rc = launch_units(3, c, in.off, out.off, bytes, 0, 0, g->stream);
+  const int blocks = grid_for(bytes / 16 + 1, 4);
+  sig_grid(c, blocks);
+  with_unit(in.off | out.off | bytes, [&](auto u) { alltoall_kernel<decltype(u), 4><<<blocks, kThreads, 0, g->stream>>>(c, in.off, out.off, bytes); });
+  rc = launch_check("alltoall_kernel");
   if (rc) return rc;
   rc = copy_out(recv, bytes * n, memkind, out);
   if (rc) return rc;
@@ -1314,28 +1300,18 @@ static int make_vtable(const char* what, const size_t* counts, size_t es, VTable
   return 0;
 }
 
-// which: 0 gather(v) / allgatherv push (peer = destination rank, -1 all), 1 scatterv pull (peer = root).
-// The grid follows the largest block of the table, so every rank launches the same one; the access
-// unit follows this rank's offsets and every displacement (the table is the same everywhere).
-template <typename U>
-static void launch_v_u(int which, Comm& c, uint64_t a, uint64_t b, const VTable& vt, int peer, cudaStream_t s) {
-  constexpr int UNROLL = 4;
+// The grid of a table-driven launch follows the largest block, so every rank launches the same one.
+static int vtable_grid(const VTable& vt) {
   size_t largest = 0;
-  for (int r = 0; r < c.n; ++r) largest = std::max<size_t>(largest, vt.off[r + 1] - vt.off[r]);
-  const int blocks = grid_for(largest / 16 + 1, UNROLL);
-  sig_grid(c, blocks);
-  if (which == 0) gatherv_push_kernel<U, UNROLL><<<blocks, kThreads, 0, s>>>(c, a, b, vt, peer);
-  else scatterv_pull_kernel<U, UNROLL><<<blocks, kThreads, 0, s>>>(c, a, b, vt, peer);
+  for (int r = 0; r < g->ctrl.n; ++r) largest = std::max<size_t>(largest, vt.off[r + 1] - vt.off[r]);
+  return grid_for(largest / 16 + 1, 4);
 }
-static int launch_v(int which, uint64_t a, uint64_t b, const VTable& vt, int peer, cudaStream_t s) {
-  Comm c = next_comm();
-  uint64_t m = a | b;
-  for (int r = 0; r <= c.n; ++r) m |= vt.off[r];
-  if ((m & 15) == 0) launch_v_u<uint4>(which, c, a, b, vt, peer, s);
-  else if ((m & 7) == 0) launch_v_u<unsigned long long>(which, c, a, b, vt, peer, s);
-  else if ((m & 3) == 0) launch_v_u<unsigned int>(which, c, a, b, vt, peer, s);
-  else launch_v_u<unsigned char>(which, c, a, b, vt, peer, s);
-  return launch_check(which == 0 ? "gatherv_push_kernel" : "scatterv_pull_kernel");
+
+// OR of the displacements off[0..n]: with this rank's offsets they pick its access unit (with_unit).
+static uint64_t vtable_bits(const VTable& vt) {
+  uint64_t m = 0;
+  for (int r = 0; r <= g->ctrl.n; ++r) m |= vt.off[r];
+  return m;
 }
 
 // A staged result is copied back only after the collective succeeded: a mismatched call
@@ -1383,8 +1359,11 @@ static int do_gatherv(const void* send, void* recv, const size_t* counts, int dt
   else if ((rc = resolve_in(send, mine, memkind, 0, in))) return rc;
   if (!gets) out = in; // announced but never written: only root's recv is a destination
   g->cur_sig = make_sig(all ? 9 : 7, dtype, root, 0, total / es, hash);
-  rc = launch_v(0, in.off, out.off, vt, root, g->stream);
-  if (rc) return rc;
+  Comm c = next_comm();
+  const int blocks = vtable_grid(vt);
+  sig_grid(c, blocks);
+  with_unit(in.off | out.off | vtable_bits(vt), [&](auto u) { gatherv_push_kernel<decltype(u), 4><<<blocks, kThreads, 0, g->stream>>>(c, in.off, out.off, vt, root); });
+  if ((rc = launch_check("gatherv_push_kernel"))) return rc;
   if (gets && (rc = copy_out_checked(recv, total, memkind, out))) return rc;
   return finish(false);
 }
@@ -1414,8 +1393,11 @@ static int do_scatterv(const void* send, void* recv, const size_t* counts, int d
   else if ((rc = resolve_out(recv, mine, memkind, 1, out))) return rc;
   if (!is_root) in = out; // announced but never read: only root's send is a source
   g->cur_sig = make_sig(8, dtype, root, 0, total / es, hash);
-  rc = launch_v(1, in.off, out.off, vt, root, g->stream);
-  if (rc) return rc;
+  Comm c = next_comm();
+  const int blocks = vtable_grid(vt);
+  sig_grid(c, blocks);
+  with_unit(in.off | out.off | vtable_bits(vt), [&](auto u) { scatterv_pull_kernel<decltype(u), 4><<<blocks, kThreads, 0, g->stream>>>(c, in.off, out.off, vt, root); });
+  if ((rc = launch_check("scatterv_pull_kernel"))) return rc;
   rc = copy_out_checked(recv, mine, memkind, out);
   if (rc) return rc;
   return finish(false);
@@ -1427,30 +1409,6 @@ static int do_gather(const void* send, void* recv, size_t count, int dtype, int 
   if (rc) return rc;
   const std::vector<size_t> counts((size_t)g->ctrl.n, count);
   return scatter ? do_scatterv(send, recv, counts.data(), dtype, root, memkind) : do_gatherv(send, recv, counts.data(), dtype, root, false, memkind);
-}
-
-// Alltoallv.  The grid is block_cap() CTAs whatever the table: the barriers pair CTAs by blockIdx and
-// the grid is part of the signature, so it may depend only on what every rank shares.  The access
-// unit follows this rank's offsets and both of its displacement tables; a peer whose offsets are less
-// aligned sends this rank to the byte-wide body (kernels.cuh).
-template <typename U>
-static void launch_alltoallv_u(Comm& c, uint64_t a, uint64_t b, const VTable& sv, const VTable& rv, uint64_t digest, cudaStream_t s) {
-  constexpr int UNROLL = 4;
-  const int blocks = block_cap();
-  sig_grid(c, blocks);
-  const uint64_t base_sig = c.sig;
-  c.sig = base_sig + digest;
-  alltoallv_push_kernel<U, UNROLL><<<blocks, kThreads, 0, s>>>(c, a, b, sv, rv, base_sig);
-}
-static int launch_alltoallv(uint64_t a, uint64_t b, const VTable& sv, const VTable& rv, uint64_t digest, cudaStream_t s) {
-  Comm c = next_comm();
-  uint64_t m = a | b;
-  for (int r = 0; r <= c.n; ++r) m |= sv.off[r] | rv.off[r];
-  if ((m & 15) == 0) launch_alltoallv_u<uint4>(c, a, b, sv, rv, digest, s);
-  else if ((m & 7) == 0) launch_alltoallv_u<unsigned long long>(c, a, b, sv, rv, digest, s);
-  else if ((m & 3) == 0) launch_alltoallv_u<unsigned int>(c, a, b, sv, rv, digest, s);
-  else launch_alltoallv_u<unsigned char>(c, a, b, sv, rv, digest, s);
-  return launch_check("alltoallv_push_kernel");
 }
 
 // Alltoallv: block j of send (send_counts[j] elements, packed in rank order) goes to rank j, where it
@@ -1478,8 +1436,17 @@ static int do_alltoallv(const void* send, const size_t* send_counts, void* recv,
   if ((rc = resolve_in(send, sbytes, memkind, 0, in))) return rc;
   if ((rc = resolve_out(recv, rbytes, memkind, 1, out))) return rc;
   g->cur_sig = make_sig(10, dtype, 0, 0, 0);
-  rc = launch_alltoallv(in.off, out.off, sv, rv, digest, g->stream);
-  if (rc) return rc;
+  // The grid is block_cap() CTAs whatever the table: the barriers pair CTAs by blockIdx and the grid
+  // is part of the signature, so it may depend only on what every rank shares.  The access unit
+  // follows this rank's offsets and both of its displacement tables.
+  Comm c = next_comm();
+  const int blocks = block_cap();
+  sig_grid(c, blocks);
+  const uint64_t base_sig = c.sig;
+  c.sig = base_sig + digest;
+  with_unit(in.off | out.off | vtable_bits(sv) | vtable_bits(rv),
+            [&](auto u) { alltoallv_push_kernel<decltype(u), 4><<<blocks, kThreads, 0, g->stream>>>(c, in.off, out.off, sv, rv, base_sig); });
+  if ((rc = launch_check("alltoallv_push_kernel"))) return rc;
   if ((rc = copy_out_checked(recv, rbytes, memkind, out))) return rc;
   return finish(false);
 }

@@ -1169,8 +1169,55 @@ __device__ __forceinline__ bool all_aligned_to(const uint64_t* s_a, const uint64
   return (m & (unit - 1)) == 0;
 }
 
-// Direct push: every rank streams its block once from local HBM and stores it into all n recv
-// buffers (own copy skipped when the call is in place).
+// The copy loop of the push and pull bodies: units [lo, hi) of src, grid-strided, UNROLL loads in
+// flight per thread, then each unit stored to the first `ntargets` of dst[0..MAXT).  push_rotated
+// keeps its own single-target loop: inside its loop over targets, this one compiled to more
+// registers.
+template <typename U, int UNROLL, int MAXT>
+__device__ __forceinline__ void copy_units(const U* src, U* const* dst, int ntargets, size_t lo, size_t hi) {
+  const size_t step = (size_t)gridDim.x * blockDim.x * UNROLL;
+  for (size_t i0 = lo + (size_t)blockIdx.x * blockDim.x * UNROLL + threadIdx.x; i0 < hi; i0 += step) {
+    U v[UNROLL];
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u) {
+      const size_t i = i0 + (size_t)u * blockDim.x;
+      if (i < hi) v[u] = src[i];
+    }
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u) {
+      const size_t i = i0 + (size_t)u * blockDim.x;
+      if (i < hi) {
+#pragma unroll
+        for (int r = 0; r < MAXT; ++r)
+          if (r < ntargets) dst[r][i] = v[u];
+      }
+    }
+  }
+}
+
+// Direct push: every rank streams its block [lo, lo + bytes) once from local HBM and stores it at lo
+// in the recv buffer of `only_dst` (Gather) or of all n ranks, own last (only_dst == -1: Allgather,
+// Allgatherv).  The own copy is skipped when the call is in place (send == recv + lo).
+template <typename U, int UNROLL>
+__device__ __forceinline__ void push_block_body(const Comm& c, const uint64_t* s_a, const uint64_t* s_b, uint64_t lo,
+                                                uint64_t bytes, int only_dst) {
+  const int n = c.n;
+  const size_t units = bytes / sizeof(U);
+  const U* src = reinterpret_cast<const U*>(c.base[c.rank] + s_a[c.rank]);
+  const bool inplace = s_a[c.rank] == s_b[c.rank] + lo;
+  U* dst[kMaxRanks];
+#pragma unroll
+  for (int r = 0; r < kMaxRanks; ++r) {
+    const int w = only_dst >= 0 ? only_dst : (c.rank + 1 + r) % n; // w == rank when r == n-1
+    dst[r] = reinterpret_cast<U*>(c.base[w] + s_b[w] + lo);
+  }
+  const int ntargets = only_dst >= 0 ? (only_dst == c.rank && inplace ? 0 : 1) : (inplace ? n - 1 : n);
+  copy_units<U, UNROLL, kMaxRanks>(src, dst, ntargets, 0, units);
+}
+
+// push_block_body with lo = rank * bytes_per_rank and every rank a target, for the P2P fallback of
+// allgather_nvls_kernel: with push_block_body that kernel compiled to 64 registers and 56 more
+// instructions than with this body.
 template <typename U, int UNROLL>
 __device__ __forceinline__ void allgather_push_body(const Comm& c, const uint64_t* s_a, const uint64_t* s_b,
                                                     size_t bytes_per_rank) {
@@ -1184,25 +1231,7 @@ __device__ __forceinline__ void allgather_push_body(const Comm& c, const uint64_
     const int w = (c.rank + 1 + r) % n; // w == rank when r == n-1
     dst[r] = reinterpret_cast<U*>(c.base[w] + s_b[w] + (size_t)c.rank * bytes_per_rank);
   }
-  const int ntargets = inplace ? n - 1 : n;
-  const size_t step = (size_t)gridDim.x * blockDim.x * UNROLL;
-  for (size_t i0 = (size_t)blockIdx.x * blockDim.x * UNROLL + threadIdx.x; i0 < units; i0 += step) {
-    U v[UNROLL];
-#pragma unroll
-    for (int u = 0; u < UNROLL; ++u) {
-      const size_t i = i0 + (size_t)u * blockDim.x;
-      if (i < units) v[u] = src[i];
-    }
-#pragma unroll
-    for (int u = 0; u < UNROLL; ++u) {
-      const size_t i = i0 + (size_t)u * blockDim.x;
-      if (i < units) {
-#pragma unroll
-        for (int r = 0; r < kMaxRanks; ++r)
-          if (r < ntargets) dst[r][i] = v[u];
-      }
-    }
-  }
+  copy_units<U, UNROLL, kMaxRanks>(src, dst, inplace ? n - 1 : n, 0, units);
 }
 
 template <typename U, int UNROLL>
@@ -1214,8 +1243,8 @@ allgather_push_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t bytes
     sync_end_failed(c);
     return;
   }
-  if (sizeof(U) == 1 || all_aligned_to(s_a, s_b, c.n, sizeof(U))) allgather_push_body<U, UNROLL>(c, s_a, s_b, bytes_per_rank);
-  else allgather_push_body<unsigned char, 1>(c, s_a, s_b, bytes_per_rank);
+  if (sizeof(U) == 1 || all_aligned_to(s_a, s_b, c.n, sizeof(U))) push_block_body<U, UNROLL>(c, s_a, s_b, (uint64_t)c.rank * bytes_per_rank, bytes_per_rank, -1);
+  else push_block_body<unsigned char, 1>(c, s_a, s_b, (uint64_t)c.rank * bytes_per_rank, bytes_per_rank, -1);
   sync_end(c);
 }
 
@@ -1297,24 +1326,7 @@ __device__ __forceinline__ void bcast_body(const Comm& c, const uint64_t* s_a, s
     }
   }
   for (int j = ntargets; j < kMaxRanks; ++j) dst[j] = dst[0];
-  const size_t step = (size_t)gridDim.x * blockDim.x * UNROLL;
-  for (size_t i0 = lo + (size_t)blockIdx.x * blockDim.x * UNROLL + threadIdx.x; i0 < hi; i0 += step) {
-    U v[UNROLL];
-#pragma unroll
-    for (int u = 0; u < UNROLL; ++u) {
-      const size_t i = i0 + (size_t)u * blockDim.x;
-      if (i < hi) v[u] = src[i];
-    }
-#pragma unroll
-    for (int u = 0; u < UNROLL; ++u) {
-      const size_t i = i0 + (size_t)u * blockDim.x;
-      if (i < hi) {
-#pragma unroll
-        for (int r = 0; r < kMaxRanks; ++r)
-          if (r < ntargets) dst[r][i] = v[u];
-      }
-    }
-  }
+  copy_units<U, UNROLL, kMaxRanks>(src, dst, ntargets, lo, hi);
 }
 
 template <typename U, int UNROLL>
@@ -1462,29 +1474,38 @@ allgather_nvls_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t bytes
 // Alltoall: block j of rank r's send buffer becomes block r of rank j's recv buffer.  Direct
 // push, n write streams per GPU, targets rotated so that the ranks do not all hit one peer.
 // ---------------------------------------------------------------------------------------------
-template <typename U, int UNROLL>
-__device__ __forceinline__ void alltoall_body(const Comm& c, const uint64_t* s_a, const uint64_t* s_b, size_t bytes_per_block) {
+// Block j of this rank's send, len(j) bytes at src(j), goes to dst(j) in rank j's heap; targets
+// rotated with the own block last (a local copy).  Each block is grid-strided over all CTAs.
+template <typename U, int UNROLL, typename Src, typename Dst, typename Len>
+__device__ __forceinline__ void push_rotated(const Comm& c, Src src, Dst dst, Len len) {
   const int n = c.n;
-  const size_t units = bytes_per_block / sizeof(U);
   const size_t step = (size_t)gridDim.x * blockDim.x * UNROLL;
   for (int k = 0; k < n; ++k) {
     const int j = (c.rank + 1 + k) % n; // own block last
-    const U* src = reinterpret_cast<const U*>(c.base[c.rank] + s_a[c.rank] + (size_t)j * bytes_per_block);
-    U* dst = reinterpret_cast<U*>(c.base[j] + s_b[j] + (size_t)c.rank * bytes_per_block);
+    const size_t units = len(j) / sizeof(U);
+    const U* s = reinterpret_cast<const U*>(src(j));
+    U* d = reinterpret_cast<U*>(dst(j));
     for (size_t i0 = (size_t)blockIdx.x * blockDim.x * UNROLL + threadIdx.x; i0 < units; i0 += step) {
       U v[UNROLL];
 #pragma unroll
       for (int u = 0; u < UNROLL; ++u) {
         const size_t i = i0 + (size_t)u * blockDim.x;
-        if (i < units) v[u] = src[i];
+        if (i < units) v[u] = s[i];
       }
 #pragma unroll
       for (int u = 0; u < UNROLL; ++u) {
         const size_t i = i0 + (size_t)u * blockDim.x;
-        if (i < units) dst[i] = v[u];
+        if (i < units) d[i] = v[u];
       }
     }
   }
+}
+
+template <typename U, int UNROLL>
+__device__ __forceinline__ void alltoall_body(const Comm& c, const uint64_t* s_a, const uint64_t* s_b, size_t bytes_per_block) {
+  push_rotated<U, UNROLL>(
+      c, [&](int j) { return c.base[c.rank] + s_a[c.rank] + (size_t)j * bytes_per_block; },
+      [&](int j) { return c.base[j] + s_b[j] + (size_t)c.rank * bytes_per_block; }, [&](int) { return bytes_per_block; });
 }
 
 template <typename U, int UNROLL>
@@ -1518,42 +1539,12 @@ __device__ __forceinline__ void vtable_range(const VTable& vt, int me, uint64_t&
     if (r == me) { lo = vt.off[r]; hi = vt.off[r + 1]; }
 }
 
-// Every rank streams its own block once from local HBM and stores it at its displacement in the
-// recv buffer of `only_dst` (Gather) or of all n ranks, own last (only_dst == -1: Allgatherv).  The
-// own copy is skipped when the call is in place (send == recv + displacement).
+// Every rank pushes its own block, at its displacement in the table (push_block_body).
 template <typename U, int UNROLL>
 __device__ __forceinline__ void gatherv_push_body(const Comm& c, const uint64_t* s_a, const uint64_t* s_b, const VTable& vt, int only_dst) {
-  const int n = c.n;
   uint64_t lo, hi;
   vtable_range(vt, c.rank, lo, hi);
-  const size_t units = (hi - lo) / sizeof(U);
-  const U* src = reinterpret_cast<const U*>(c.base[c.rank] + s_a[c.rank]);
-  const bool inplace = s_a[c.rank] == s_b[c.rank] + lo;
-  U* dst[kMaxRanks];
-#pragma unroll
-  for (int r = 0; r < kMaxRanks; ++r) {
-    const int w = only_dst >= 0 ? only_dst : (c.rank + 1 + r) % n; // w == rank when r == n-1
-    dst[r] = reinterpret_cast<U*>(c.base[w] + s_b[w] + lo);
-  }
-  const int ntargets = only_dst >= 0 ? (only_dst == c.rank && inplace ? 0 : 1) : (inplace ? n - 1 : n);
-  const size_t step = (size_t)gridDim.x * blockDim.x * UNROLL;
-  for (size_t i0 = (size_t)blockIdx.x * blockDim.x * UNROLL + threadIdx.x; i0 < units; i0 += step) {
-    U v[UNROLL];
-#pragma unroll
-    for (int u = 0; u < UNROLL; ++u) {
-      const size_t i = i0 + (size_t)u * blockDim.x;
-      if (i < units) v[u] = src[i];
-    }
-#pragma unroll
-    for (int u = 0; u < UNROLL; ++u) {
-      const size_t i = i0 + (size_t)u * blockDim.x;
-      if (i < units) {
-#pragma unroll
-        for (int r = 0; r < kMaxRanks; ++r)
-          if (r < ntargets) dst[r][i] = v[u];
-      }
-    }
-  }
+  push_block_body<U, UNROLL>(c, s_a, s_b, lo, hi - lo, only_dst);
 }
 
 template <typename U, int UNROLL>
@@ -1580,21 +1571,8 @@ __device__ __forceinline__ void scatterv_pull_body(const Comm& c, const uint64_t
   if (c.rank == root && s_b[root] == s_a[root] + lo) return;
   const size_t units = (hi - lo) / sizeof(U);
   const U* src = reinterpret_cast<const U*>(c.base[root] + s_a[root] + lo);
-  U* dst = reinterpret_cast<U*>(c.base[c.rank] + s_b[c.rank]);
-  const size_t step = (size_t)gridDim.x * blockDim.x * UNROLL;
-  for (size_t i0 = (size_t)blockIdx.x * blockDim.x * UNROLL + threadIdx.x; i0 < units; i0 += step) {
-    U v[UNROLL];
-#pragma unroll
-    for (int u = 0; u < UNROLL; ++u) {
-      const size_t i = i0 + (size_t)u * blockDim.x;
-      if (i < units) v[u] = src[i];
-    }
-#pragma unroll
-    for (int u = 0; u < UNROLL; ++u) {
-      const size_t i = i0 + (size_t)u * blockDim.x;
-      if (i < units) dst[i] = v[u];
-    }
-  }
+  U* const dst = reinterpret_cast<U*>(c.base[c.rank] + s_b[c.rank]);
+  copy_units<U, UNROLL, 1>(src, &dst, 1, 0, units);
 }
 
 template <typename U, int UNROLL>
@@ -1650,32 +1628,11 @@ __host__ __device__ inline bool a2av_tables(int me, int n, const size_t* send_co
 }
 
 // Push: every rank reads its n send blocks once from local HBM and stores block j at s_b[j] of rank
-// j's heap, targets rotated with the own block last (a local copy).  Each target's range is
-// grid-strided over all CTAs, so a skewed table still spreads over the whole grid.  s_src[j] is the
+// j's heap (push_rotated), so a skewed table still spreads over the whole grid.  s_src[j] is the
 // heap offset of block j in this rank's send, s_len[j] its bytes.
 template <typename U, int UNROLL>
 __device__ __forceinline__ void alltoallv_push_body(const Comm& c, const uint64_t* s_src, const uint64_t* s_len, const uint64_t* s_b) {
-  const int n = c.n;
-  const size_t step = (size_t)gridDim.x * blockDim.x * UNROLL;
-  for (int k = 0; k < n; ++k) {
-    const int j = (c.rank + 1 + k) % n;
-    const size_t units = s_len[j] / sizeof(U);
-    const U* src = reinterpret_cast<const U*>(c.base[c.rank] + s_src[j]);
-    U* dst = reinterpret_cast<U*>(c.base[j] + s_b[j]);
-    for (size_t i0 = (size_t)blockIdx.x * blockDim.x * UNROLL + threadIdx.x; i0 < units; i0 += step) {
-      U v[UNROLL];
-#pragma unroll
-      for (int u = 0; u < UNROLL; ++u) {
-        const size_t i = i0 + (size_t)u * blockDim.x;
-        if (i < units) v[u] = src[i];
-      }
-#pragma unroll
-      for (int u = 0; u < UNROLL; ++u) {
-        const size_t i = i0 + (size_t)u * blockDim.x;
-        if (i < units) dst[i] = v[u];
-      }
-    }
-  }
+  push_rotated<U, UNROLL>(c, [&](int j) { return c.base[c.rank] + s_src[j]; }, [&](int j) { return c.base[j] + s_b[j]; }, [&](int j) { return s_len[j]; });
 }
 
 // sv / rv: this rank's send and recv displacements (a2av_tables); c.sig = base_sig + its digest.

@@ -522,6 +522,13 @@ def scenario_unaligned(a):
                 check_equal(wb.to_host(), wins[root], "mixed-width bcast %s %s" % (dn, algo))
                 done += 1
             lib.b200mpi_set_algo(L.COLL_BCAST, 0)
+            # Alltoall blocks of big_n / n elements (a multiple of 16 bytes); send and recv both sit
+            # 8/16/24 bytes in, so the 16-byte-aligned ranks see a narrower peer and run the byte body
+            wa = wsrc[so:so + big_n].copy_from_host(wins[rank])
+            wt = wide[so:so + big_n]
+            mpi.Alltoall(wa, wt)
+            check_equal(wt.to_host(), O.alltoall(wins, rank), "mixed-width alltoall %s" % dn)
+            done += 1
             wide.free()
             wsrc.free()
         # bytes: odd length, odd offset

@@ -39,7 +39,8 @@ def free_ports(n):
     raise RuntimeError("no run of %d free ports found" % n)
 
 
-def run_world(n, scenario, args=(), env=None, timeout=600, gpus_shared=True, extra_flags=(), per_rank_env=None):
+def run_world(n, scenario, args=(), env=None, timeout=600, gpus_shared=True, extra_flags=(), per_rank_env=None, worker=None):
+    """worker: the rank program (default WORKER, _worker.py)."""
     ports = free_ports(n)
     addrs = ["127.0.0.1:%d" % p for p in ports]
     procs = []
@@ -56,7 +57,7 @@ def run_world(n, scenario, args=(), env=None, timeout=600, gpus_shared=True, ext
         er = dict(e)
         if per_rank_env:
             er.update(per_rank_env(r))
-        cmd = [sys.executable, WORKER, scenario, "--out", outs[r]] + list(args) + list(extra_flags) + [
+        cmd = [sys.executable, worker or WORKER, scenario, "--out", outs[r]] + list(args) + list(extra_flags) + [
             "-mpi-addr", addrs[r], "-mpi-alladdr", ",".join(addrs), "-mpi-inittimeout", "60s"]
         procs.append(subprocess.Popen(cmd, env=er, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True))
     # A rank that fails leaves its peers blocked in a collective: give them a short grace period,

@@ -101,7 +101,6 @@ struct Ctx {
   Comm comm = {};
   uint32_t epoch = 1;
   uint32_t scrub_every = kScrubEvery; // power of two; B200MPI_SCRUB_EVERY lowers it so that a test can reach the scrub
-  uint64_t cur_sig = 0; // signature of the collective being launched (checked by sync_start on every rank)
   uint32_t* status_host = nullptr; // mapped pinned
   uint32_t* status_dev = nullptr;
   cudaStream_t own_stream = nullptr, stream = nullptr;
@@ -258,8 +257,9 @@ static int grid_for(size_t units_per_rank, int unroll) {
 }
 
 // Every launch advances the epoch by kEpochStride whatever the algorithm (kernels.cuh), so ranks
-// that disagreed about one call still agree about the flag values of the next.
-static Comm next_comm() {
+// that disagreed about one call still agree about the flag values of the next.  `sig` is what this
+// rank thinks the call is (make_sig), checked by sync_start on every rank.
+static Comm next_comm(uint64_t sig) {
   // Every kScrubEvery-th launch (the same one on every rank: epochs move in lockstep) is preceded by
   // scrub_kernel, which rewrites every slot row so that no flag word can fall 2^31 behind the epoch.
   if (g->ctrl.n > 1 && ((g->epoch / kEpochStride) & (g->scrub_every - 1)) == g->scrub_every - 1) {
@@ -273,7 +273,7 @@ static Comm next_comm() {
   }
   Comm c = g->comm;
   c.epoch = g->epoch;
-  c.sig = g->cur_sig;
+  c.sig = sig;
   c.end_epoch = g->epoch + kEpochStride - 1;
   g->epoch += kEpochStride;
   return c;
@@ -337,6 +337,17 @@ static int launch_check(const char* what) {
   return 0;
 }
 
+// One collective launch: take the epoch, fold the grid into the signature, launch kernel(comm,
+// args...) and check the launch.  Callers settle the algorithm and the grid first, so a launch that
+// does not happen takes no epoch.
+template <typename... P, typename... A>
+static int launch_coll(void (*kernel)(Comm, P...), const char* what, uint64_t sig, int blocks, int threads, size_t smem, cudaStream_t s, A... args) {
+  Comm c = next_comm(sig);
+  sig_grid(c, blocks);
+  kernel<<<blocks, threads, smem, s>>>(c, args...);
+  return launch_check(what);
+}
+
 // dst <- src on `s` with the library's own copy kernel (local HBM or peer mapping), any alignment:
 // 256 threads x 16 vectors in flight per thread, up to one CTA per SM (or max_blocks).
 static int launch_copy(void* dst, const void* src, size_t bytes, cudaStream_t s) {
@@ -381,21 +392,16 @@ static uint32_t own_shift(size_t nvec, int n, uint32_t min_shift) {
 
 // only_dst: -1 allreduce, else the root of a Reduce (twoshot / nvls only)
 template <typename T, typename Op>
-static int launch_allreduce_body_t(int algo, uint64_t so, uint64_t ro, size_t count, int only_dst, cudaStream_t s) {
+static int launch_allreduce_body_t(int algo, uint64_t sig, uint64_t so, uint64_t ro, size_t count, int only_dst, cudaStream_t s) {
   const int n = g->ctrl.n;
   constexpr int EPV = 16 / sizeof(T);
   const size_t nvec = (count + EPV - 1) / EPV;
   const size_t per = (nvec + n - 1) / n;
   const uint32_t sh = own_shift(nvec, n, algo == B200MPI_ALGO_TWOSHOT_SMEM ? 8 : 0);
-  Comm c = next_comm();
   switch (algo) {
     case B200MPI_ALGO_TWOSHOT: {
-#define B200_TWOSHOT(NRV, UV)                                                                          \
-  {                                                                                                    \
-    const int blocks = grid_for(per, UV);                                                              \
-    sig_grid(c, blocks);                                                                               \
-    allreduce_twoshot_kernel<T, Op, NRV, UV><<<blocks, kThreads, 0, s>>>(c, so, ro, count, sh, only_dst); \
-  }
+#define B200_TWOSHOT(NRV, UV) \
+  return launch_coll(allreduce_twoshot_kernel<T, Op, NRV, UV>, "allreduce_twoshot_kernel", sig, grid_for(per, UV), kThreads, 0, s, so, ro, count, sh, only_dst);
       if (g->twoshot_unroll) {
         if (n == 2) B200_TWOSHOT(2, (sizeof(T) == 4 ? 8 : 4)) // 8-byte min/max spilled at 8 vectors per thread
         else if (n == 4) B200_TWOSHOT(4, 4)
@@ -408,18 +414,12 @@ static int launch_allreduce_body_t(int algo, uint64_t so, uint64_t ro, size_t co
         else B200_TWOSHOT(0, 1)
       }
 #undef B200_TWOSHOT
-      return launch_check("allreduce_twoshot_kernel");
     }
-    case B200MPI_ALGO_RING: {
-      const int blocks = grid_for(per, 4);
-      sig_grid(c, blocks);
-      allreduce_ring_kernel<T, Op><<<blocks, kThreads, 0, s>>>(c, so, ro, count);
-      return launch_check("allreduce_ring_kernel");
-    }
+    case B200MPI_ALGO_RING:
+      return launch_coll(allreduce_ring_kernel<T, Op>, "allreduce_ring_kernel", sig, grid_for(per, 4), kThreads, 0, s, so, ro, count);
     case B200MPI_ALGO_TWOSHOT_SMEM: {
       const size_t tiles = (per * 16 + kSmemChunk - 1) / kSmemChunk;
       const int blocks = (int)std::max<size_t>(1, std::min<size_t>(tiles, (size_t)block_cap()));
-      sig_grid(c, blocks);
 #define B200_SMEM(NRV)                                                                                           \
   {                                                                                                              \
     const size_t smem = (size_t)(kSmemStages * NRV + kSmemOutStages) * kSmemChunk;                               \
@@ -428,13 +428,12 @@ static int launch_allreduce_body_t(int algo, uint64_t so, uint64_t ro, size_t co
       cudaFuncSetAttribute(allreduce_twoshot_smem_kernel<T, Op, NRV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
       attr_set = true;                                                                                           \
     }                                                                                                            \
-    allreduce_twoshot_smem_kernel<T, Op, NRV><<<blocks, kSmemThreads, smem, s>>>(c, so, ro, count, sh);              \
+    return launch_coll(allreduce_twoshot_smem_kernel<T, Op, NRV>, "allreduce_twoshot_smem_kernel", sig, blocks, kSmemThreads, smem, s, so, ro, count, sh); \
   }
       if (n == 2) B200_SMEM(2)
       else if (n == 4) B200_SMEM(4)
       else B200_SMEM(8)
 #undef B200_SMEM
-      return launch_check("allreduce_twoshot_smem_kernel");
     }
   }
   return fail(B200MPI_ERR_UNSUPPORTED, "allreduce: algorithm not available for this dtype/op");
@@ -457,25 +456,21 @@ static OneshotPlan oneshot_plan(size_t count, size_t es) {
 }
 
 template <typename T, typename Op>
-static int launch_allreduce_t(int algo, uint64_t so, uint64_t ro, size_t count, cudaStream_t s) {
+static int launch_allreduce_t(int algo, uint64_t sig, uint64_t so, uint64_t ro, size_t count, cudaStream_t s) {
   const int n = g->ctrl.n;
-  if (algo != B200MPI_ALGO_ONESHOT) return launch_allreduce_body_t<T, Op>(algo, so, ro, count, -1, s);
+  if (algo != B200MPI_ALGO_ONESHOT) return launch_allreduce_body_t<T, Op>(algo, sig, so, ro, count, -1, s);
   const OneshotPlan p = oneshot_plan(count, sizeof(T));
   if (p.rounds > kMaxMids) return fail(B200MPI_ERR_UNSUPPORTED, "allreduce: message too large for the one-shot algorithm");
-  Comm c = next_comm();
-  sig_grid(c, p.blocks);
-  const int blocks = p.blocks;
+  auto go = [&](auto kernel, const char* what) { return launch_coll(kernel, what, sig, p.blocks, kThreads, 0, s, so, ro, count); };
   if (p.shfl) {
-    if (n == 2) allreduce_oneshot_shfl_kernel<T, Op, 2><<<blocks, kThreads, 0, s>>>(c, so, ro, count);
-    else if (n == 4) allreduce_oneshot_shfl_kernel<T, Op, 4><<<blocks, kThreads, 0, s>>>(c, so, ro, count);
-    else allreduce_oneshot_shfl_kernel<T, Op, 8><<<blocks, kThreads, 0, s>>>(c, so, ro, count);
-    return launch_check("allreduce_oneshot_shfl_kernel");
+    if (n == 2) return go(allreduce_oneshot_shfl_kernel<T, Op, 2>, "allreduce_oneshot_shfl_kernel");
+    if (n == 4) return go(allreduce_oneshot_shfl_kernel<T, Op, 4>, "allreduce_oneshot_shfl_kernel");
+    return go(allreduce_oneshot_shfl_kernel<T, Op, 8>, "allreduce_oneshot_shfl_kernel");
   }
-  if (n == 2) allreduce_oneshot_kernel<T, Op, 2><<<blocks, kThreads, 0, s>>>(c, so, ro, count);
-  else if (n == 4) allreduce_oneshot_kernel<T, Op, 4><<<blocks, kThreads, 0, s>>>(c, so, ro, count);
-  else if (n == 8) allreduce_oneshot_kernel<T, Op, 8><<<blocks, kThreads, 0, s>>>(c, so, ro, count);
-  else allreduce_oneshot_kernel<T, Op, 0><<<blocks, kThreads, 0, s>>>(c, so, ro, count);
-  return launch_check("allreduce_oneshot_kernel");
+  if (n == 2) return go(allreduce_oneshot_kernel<T, Op, 2>, "allreduce_oneshot_kernel");
+  if (n == 4) return go(allreduce_oneshot_kernel<T, Op, 4>, "allreduce_oneshot_kernel");
+  if (n == 8) return go(allreduce_oneshot_kernel<T, Op, 8>, "allreduce_oneshot_kernel");
+  return go(allreduce_oneshot_kernel<T, Op, 0>, "allreduce_oneshot_kernel");
 }
 
 static int nvls_blocks(size_t per, int u) {
@@ -485,29 +480,27 @@ static int nvls_blocks(size_t per, int u) {
 }
 
 template <typename T, typename Op>
-static int launch_allreduce_nvls_t(uint64_t so, uint64_t ro, size_t count, int only_dst, cudaStream_t s) {
-  Comm c = next_comm();
+static int launch_allreduce_nvls_t(uint64_t sig, uint64_t so, uint64_t ro, size_t count, int only_dst, cudaStream_t s) {
+  const int n = g->ctrl.n;
   constexpr int EPV = 16 / sizeof(T);
   const size_t nvec = (count + EPV - 1) / EPV;
-  const size_t per = (nvec + c.n - 1) / c.n;
-  const uint32_t sh = own_shift(nvec, c.n, 0);
+  const size_t per = (nvec + n - 1) / n;
+  const uint32_t sh = own_shift(nvec, n, 0);
   int u = g->nvls_unroll;
   if (u != 1 && u != 2 && u != 8) u = 4;
-  const int blocks = nvls_blocks(per, u);
-  sig_grid(c, blocks);
+  auto go = [&](auto kernel) { return launch_coll(kernel, "allreduce_nvls_kernel", sig, nvls_blocks(per, u), kThreads, 0, s, so, ro, count, sh, only_dst); };
   switch (u) {
-    case 1: allreduce_nvls_kernel<T, Op, 1><<<blocks, kThreads, 0, s>>>(c, so, ro, count, sh, only_dst); break;
-    case 2: allreduce_nvls_kernel<T, Op, 2><<<blocks, kThreads, 0, s>>>(c, so, ro, count, sh, only_dst); break;
-    case 8: allreduce_nvls_kernel<T, Op, 8><<<blocks, kThreads, 0, s>>>(c, so, ro, count, sh, only_dst); break;
-    default: allreduce_nvls_kernel<T, Op, 4><<<blocks, kThreads, 0, s>>>(c, so, ro, count, sh, only_dst); break;
+    case 1: return go(allreduce_nvls_kernel<T, Op, 1>);
+    case 2: return go(allreduce_nvls_kernel<T, Op, 2>);
+    case 8: return go(allreduce_nvls_kernel<T, Op, 8>);
   }
-  return launch_check("allreduce_nvls_kernel");
+  return go(allreduce_nvls_kernel<T, Op, 4>);
 }
 
 // NVLS for [0, split) + fused P2P two-shot for the rest, in one kernel (kernels.cuh).  The split is
 // cut on ownership-block boundaries of both parts and depends on (count, n, parameters) only.
 template <typename T, typename Op>
-static int launch_allreduce_hybrid_t(uint64_t so, uint64_t ro, size_t count, cudaStream_t s) {
+static int launch_allreduce_hybrid_t(uint64_t sig, uint64_t so, uint64_t ro, size_t count, cudaStream_t s) {
   const int n = g->ctrl.n;
   constexpr int EPV = 16 / sizeof(T);
   const size_t nvec = count / EPV; // whole vectors; the tail goes with the P2P part
@@ -516,24 +509,21 @@ static int launch_allreduce_hybrid_t(uint64_t so, uint64_t ro, size_t count, cud
   p2p_vec = p2p_vec / gran * gran;
   const size_t split = nvec - p2p_vec;
   if (n != 8 && n != 4 && n != 2) return fail(B200MPI_ERR_UNSUPPORTED, "allreduce: the hybrid algorithm needs 2, 4 or 8 ranks");
-  if (split == 0 || p2p_vec == 0) return launch_allreduce_nvls_t<T, Op>(so, ro, count, -1, s);
-  Comm c = next_comm();
+  if (split == 0 || p2p_vec == 0) return launch_allreduce_nvls_t<T, Op>(sig, so, ro, count, -1, s);
   const uint32_t sh_n = own_shift(split, n, 0), sh_p = own_shift(p2p_vec, n, 0);
   int u = g->nvls_unroll == 4 ? 4 : 2;
   const int nb_nvls = nvls_blocks((split + n - 1) / n, u);
   int nb_p2p = g->hybrid_p2p_blocks > 0 ? g->hybrid_p2p_blocks : block_cap() - nb_nvls;
   nb_p2p = std::max(1, std::min(nb_p2p, block_cap() - nb_nvls));
-  if (nb_nvls + nb_p2p > block_cap()) return launch_allreduce_nvls_t<T, Op>(so, ro, count, -1, s);
-  const int blocks = nb_nvls + nb_p2p;
-  sig_grid(c, blocks);
-#define B200_HYB(NRV, UP)                                                                                                                         \
-  if (u == 4) allreduce_hybrid_kernel<T, Op, NRV, 4, UP><<<blocks, kThreads, 0, s>>>(c, so, ro, count, sh_n, sh_p, split, (unsigned)nb_nvls); \
-  else allreduce_hybrid_kernel<T, Op, NRV, 2, UP><<<blocks, kThreads, 0, s>>>(c, so, ro, count, sh_n, sh_p, split, (unsigned)nb_nvls);
-  if (n == 8) { B200_HYB(8, 2) }
-  else if (n == 4) { B200_HYB(4, 4) }
-  else { B200_HYB(2, 4) }
+  if (nb_nvls + nb_p2p > block_cap()) return launch_allreduce_nvls_t<T, Op>(sig, so, ro, count, -1, s);
+  auto go = [&](auto kernel) {
+    return launch_coll(kernel, "allreduce_hybrid_kernel", sig, nb_nvls + nb_p2p, kThreads, 0, s, so, ro, count, sh_n, sh_p, split, (unsigned)nb_nvls);
+  };
+#define B200_HYB(NRV, UP) return u == 4 ? go(allreduce_hybrid_kernel<T, Op, NRV, 4, UP>) : go(allreduce_hybrid_kernel<T, Op, NRV, 2, UP>);
+  if (n == 8) B200_HYB(8, 2)
+  if (n == 4) B200_HYB(4, 4)
+  B200_HYB(2, 4)
 #undef B200_HYB
-  return launch_check("allreduce_hybrid_kernel");
 }
 
 // The reductions the kernels are instantiated for: f32, f64 and i64 with sum, max and min.  Returns
@@ -568,7 +558,7 @@ static bool nvls_supports(int dtype, int op) {
 
 // `total`: element count of the whole user call when this launch is one chunk of it, else 0.
 static int launch_allreduce(int algo, int dtype, int op, uint64_t so, uint64_t ro, size_t count, cudaStream_t s, size_t total = 0) {
-  g->cur_sig = make_sig(0, dtype, op, algo, count, total);
+  const uint64_t sig = make_sig(0, dtype, op, algo, count, total);
   const bool nvls = algo == B200MPI_ALGO_NVLS || algo == B200MPI_ALGO_HYBRID;
   const char* nvls_only = "allreduce: NVLS supports sum (f32,f64,i64) and min/max (i64) only";
   return with_reduction(
@@ -576,9 +566,9 @@ static int launch_allreduce(int algo, int dtype, int op, uint64_t so, uint64_t r
       [&](auto t, auto o) {
         using T = decltype(t);
         using Op = decltype(o);
-        if (!nvls) return launch_allreduce_t<T, Op>(algo, so, ro, count, s);
+        if (!nvls) return launch_allreduce_t<T, Op>(algo, sig, so, ro, count, s);
         if constexpr (switch_reduces<T, Op>())
-          return algo == B200MPI_ALGO_HYBRID ? launch_allreduce_hybrid_t<T, Op>(so, ro, count, s) : launch_allreduce_nvls_t<T, Op>(so, ro, count, -1, s);
+          return algo == B200MPI_ALGO_HYBRID ? launch_allreduce_hybrid_t<T, Op>(sig, so, ro, count, s) : launch_allreduce_nvls_t<T, Op>(sig, so, ro, count, -1, s);
         else return fail(B200MPI_ERR_UNSUPPORTED, nvls_only);
       },
       [&] { return fail(B200MPI_ERR_UNSUPPORTED, nvls ? nvls_only : "allreduce: unsupported dtype/op (need f32, f64 or i64 with sum/max/min)"); });
@@ -586,49 +576,32 @@ static int launch_allreduce(int algo, int dtype, int op, uint64_t so, uint64_t r
 
 // Reduce to `root`: the owner-reduces bodies with a single destination.
 static int launch_reduce(int algo, int dtype, int op, uint64_t so, uint64_t ro, size_t count, int root, cudaStream_t s) {
-  g->cur_sig = make_sig(5, dtype, op | (root << 4), algo, count);
+  const uint64_t sig = make_sig(5, dtype, op | (root << 4), algo, count);
   return with_reduction(
       dtype, op,
       [&](auto t, auto o) {
         using T = decltype(t);
         using Op = decltype(o);
-        if (algo != B200MPI_ALGO_NVLS) return launch_allreduce_body_t<T, Op>(B200MPI_ALGO_TWOSHOT, so, ro, count, root, s);
-        if constexpr (switch_reduces<T, Op>()) return launch_allreduce_nvls_t<T, Op>(so, ro, count, root, s);
+        if (algo != B200MPI_ALGO_NVLS) return launch_allreduce_body_t<T, Op>(B200MPI_ALGO_TWOSHOT, sig, so, ro, count, root, s);
+        if constexpr (switch_reduces<T, Op>()) return launch_allreduce_nvls_t<T, Op>(sig, so, ro, count, root, s);
         else return fail(B200MPI_ERR_UNSUPPORTED, "reduce: NVLS supports sum (f32,f64,i64) and min/max (i64) only");
       },
       [] { return fail(B200MPI_ERR_UNSUPPORTED, "reduce: unsupported dtype/op (need f32, f64 or i64 with sum/max/min)"); });
 }
 
-template <typename T, typename Op>
-static int launch_reduce_scatter_p2p_t(uint64_t so, uint64_t ro, size_t count, cudaStream_t s) {
-  Comm c = next_comm();
-  constexpr int EPV = 16 / sizeof(T);
-  const int blocks = grid_for((count + EPV - 1) / EPV, 2);
-  sig_grid(c, blocks);
-  reduce_scatter_kernel<T, Op, 2><<<blocks, kThreads, 0, s>>>(c, so, ro, count);
-  return launch_check("reduce_scatter_kernel");
-}
-template <typename T> // the switch form: sums only
-static int launch_reduce_scatter_nvls_t(uint64_t so, uint64_t ro, size_t count, cudaStream_t s) {
-  Comm c = next_comm();
-  constexpr int EPV = 16 / sizeof(T);
-  const int blocks = nvls_blocks((count + EPV - 1) / EPV, 2);
-  sig_grid(c, blocks);
-  reduce_scatter_nvls_kernel<T, OpSum, 2><<<blocks, kThreads, 0, s>>>(c, so, ro, count);
-  return launch_check("reduce_scatter_nvls_kernel");
-}
-
 static int launch_reduce_scatter(int algo, int dtype, int op, uint64_t so, uint64_t ro, size_t count, cudaStream_t s) {
   const bool nvls = algo == B200MPI_ALGO_NVLS && op == B200MPI_SUM; // the switch form is instantiated for sums
-  g->cur_sig = make_sig(4, dtype, op, nvls ? B200MPI_ALGO_NVLS : B200MPI_ALGO_TWOSHOT, count);
+  const uint64_t sig = make_sig(4, dtype, op, nvls ? B200MPI_ALGO_NVLS : B200MPI_ALGO_TWOSHOT, count);
   return with_reduction(
       dtype, op,
       [&](auto t, auto o) {
         using T = decltype(t);
         using Op = decltype(o);
+        constexpr int EPV = 16 / sizeof(T);
+        const size_t nvec = (count + EPV - 1) / EPV;
         if constexpr (std::is_same<Op, OpSum>::value)
-          if (nvls) return launch_reduce_scatter_nvls_t<T>(so, ro, count, s);
-        return launch_reduce_scatter_p2p_t<T, Op>(so, ro, count, s);
+          if (nvls) return launch_coll(reduce_scatter_nvls_kernel<T, OpSum, 2>, "reduce_scatter_nvls_kernel", sig, nvls_blocks(nvec, 2), kThreads, 0, s, so, ro, count);
+        return launch_coll(reduce_scatter_kernel<T, Op, 2>, "reduce_scatter_kernel", sig, grid_for(nvec, 2), kThreads, 0, s, so, ro, count);
       },
       [&] {
         const bool known_dtype = dtype == B200MPI_F32 || dtype == B200MPI_F64 || dtype == B200MPI_I64;
@@ -699,65 +672,50 @@ static int pick_reduce_scatter(size_t, int dtype, int op) {
   return can && g->ctrl.n >= g->nvls_min_ranks ? B200MPI_ALGO_NVLS : B200MPI_ALGO_TWOSHOT;
 }
 
-// Calls f(U{}) with the widest access unit U (uint4, 8, 4 or 1 byte) dividing m, the OR of THIS
+// Returns f(U{}) for the widest access unit U (uint4, 8, 4 or 1 byte) dividing m, the OR of THIS
 // rank's offsets, sizes and displacements.  Peers may be aligned differently: after the start
 // barrier every rank knows all offsets and drops to the byte-wide body if some peer's are narrower
 // than its own unit (kernels.cuh: all_aligned_to).  Ranks may so instantiate different units but
 // must launch the same number of CTAs, because the barriers pair CTAs by blockIdx: a grid never
 // depends on U.
 template <typename F>
-static void with_unit(uint64_t m, F&& f) {
-  if ((m & 15) == 0) f(uint4{});
-  else if ((m & 7) == 0) f(0ull);
-  else if ((m & 3) == 0) f(0u);
-  else f((unsigned char)0);
+static int with_unit(uint64_t m, F&& f) {
+  if ((m & 15) == 0) return f(uint4{});
+  if ((m & 7) == 0) return f(0ull);
+  if ((m & 3) == 0) return f(0u);
+  return f((unsigned char)0);
 }
 
 // Bcast of `bytes` at heap offset `off` on every... (each rank passes its own offset)
 static int launch_bcast(int algo, int dtype, size_t count, uint64_t off, size_t bytes, int root, cudaStream_t s, size_t total = 0) {
-  g->cur_sig = make_sig(1, dtype, root, algo, count, total);
-  Comm c = next_comm();
+  const uint64_t sig = make_sig(1, dtype, root, algo, count, total);
+  const int n = g->ctrl.n;
   const size_t nvec = bytes / 16 + 1;
   if (algo == B200MPI_ALGO_NVLS) {
-    if (g->bcast_nvls2) {
-      const size_t per = (nvec + c.n - 1) / c.n;
-      const int blocks = grid_for(per, 4);
-      sig_grid(c, blocks);
-      bcast_nvls2_kernel<4><<<blocks, kThreads, 0, s>>>(c, off, bytes, root, own_shift(nvec, c.n, 0));
-      return launch_check("bcast_nvls2_kernel");
-    }
-    const int blocks = grid_for(nvec, 4);
-    sig_grid(c, blocks);
-    bcast_nvls_kernel<4><<<blocks, kThreads, 0, s>>>(c, off, bytes, root);
-    return launch_check("bcast_nvls_kernel");
+    if (g->bcast_nvls2)
+      return launch_coll(bcast_nvls2_kernel<4>, "bcast_nvls2_kernel", sig, grid_for((nvec + n - 1) / n, 4), kThreads, 0, s, off, bytes, root, own_shift(nvec, n, 0));
+    return launch_coll(bcast_nvls_kernel<4>, "bcast_nvls_kernel", sig, grid_for(nvec, 4), kThreads, 0, s, off, bytes, root);
   }
   const int mode = algo == B200MPI_ALGO_TWOSHOT ? 1 : 0; // two-shot: each non-root moves one slice
-  const int blocks = grid_for(mode ? nvec / (size_t)(c.n - 1) + 1 : nvec, 4);
-  sig_grid(c, blocks);
-  with_unit(off | bytes, [&](auto u) { bcast_kernel<decltype(u), 4><<<blocks, kThreads, 0, s>>>(c, off, bytes, root, mode); });
-  return launch_check("bcast_kernel");
+  const int blocks = grid_for(mode ? nvec / (size_t)(n - 1) + 1 : nvec, 4);
+  return with_unit(off | bytes, [&](auto u) { return launch_coll(bcast_kernel<decltype(u), 4>, "bcast_kernel", sig, blocks, kThreads, 0, s, off, bytes, root, mode); });
 }
 
 static int launch_allgather(int algo, int dtype, size_t count, uint64_t in_off, uint64_t out_off, size_t bytes, cudaStream_t s, size_t total = 0) {
-  g->cur_sig = make_sig(2, dtype, 0, algo, count, total);
-  Comm c = next_comm();
+  const uint64_t sig = make_sig(2, dtype, 0, algo, count, total);
   const int blocks = grid_for(bytes / 16 + 1, 4);
-  sig_grid(c, blocks);
-  if (algo == B200MPI_ALGO_NVLS) {
-    allgather_nvls_kernel<4><<<blocks, kThreads, 0, s>>>(c, in_off, out_off, bytes);
-    return launch_check("allgather_nvls_kernel");
-  }
-  with_unit(in_off | out_off | bytes, [&](auto u) {
+  if (algo == B200MPI_ALGO_NVLS) return launch_coll(allgather_nvls_kernel<4>, "allgather_nvls_kernel", sig, blocks, kThreads, 0, s, in_off, out_off, bytes);
+  return with_unit(in_off | out_off | bytes, [&](auto u) {
     using U = decltype(u);
-    if (algo == B200MPI_ALGO_RING) allgather_ring_kernel<U><<<blocks, kThreads, 0, s>>>(c, in_off, out_off, bytes);
-    else allgather_push_kernel<U, 4><<<blocks, kThreads, 0, s>>>(c, in_off, out_off, bytes);
+    if (algo == B200MPI_ALGO_RING) return launch_coll(allgather_ring_kernel<U>, "allgather kernel", sig, blocks, kThreads, 0, s, in_off, out_off, bytes);
+    return launch_coll(allgather_push_kernel<U, 4>, "allgather kernel", sig, blocks, kThreads, 0, s, in_off, out_off, bytes);
   });
-  return launch_check("allgather kernel");
 }
 
 // ---------------------------------------------------------------------------------------------
 // buffer resolution: heap-resident device memory is used in place; anything else (host slices,
-// foreign device pointers) is staged through a heap block on the collective stream.
+// foreign device pointers) is staged through a heap block on the collective stream, block 0 for
+// the send side and block 1 for the recv side.
 // ---------------------------------------------------------------------------------------------
 static int ensure_stage(int which, size_t bytes) {
   if (g->stage_len[which] >= bytes && bytes > 0) return 0;
@@ -795,48 +753,81 @@ static int stage_copy(void* dst, const void* src, size_t bytes, const void* fore
   return on_this_gpu(foreign, bytes) ? launch_local_copy(dst, src, bytes, g->stream) : launch_copy(dst, src, bytes, g->stream);
 }
 
-static int resolve_in(const void* p, size_t bytes, int memkind, int which, Buf& out) {
+// [p, p + bytes) as an offset in this rank's heap: where it lies, or staging block `which`, which is
+// filled from p when `fill`.
+static int resolve(const void* p, size_t bytes, int memkind, int which, bool fill, Buf& b) {
   size_t off;
   if (memkind == B200MPI_DEVICE && g->heap.contains(p, bytes, off)) {
-    out.off = off;
-    out.staged = false;
+    b = {off, false};
     return 0;
   }
-  int rc = ensure_stage(which, bytes);
+  const int rc = ensure_stage(which, bytes);
   if (rc) return rc;
-  out.off = g->stage_off[which];
-  out.staged = true;
-  if (bytes) {
-    char* dst = (char*)g->heap.base[g->ctrl.rank] + out.off;
-    if (memkind == B200MPI_HOST) CUDA_OK(cudaMemcpyAsync(dst, p, bytes, cudaMemcpyHostToDevice, g->stream));
-    else { rc = stage_copy(dst, p, bytes, p); if (rc) return rc; }
+  b = {g->stage_off[which], true};
+  if (!fill || bytes == 0) return 0;
+  char* dst = (char*)g->heap.base[g->ctrl.rank] + b.off;
+  if (memkind == B200MPI_HOST) CUDA_OK(cudaMemcpyAsync(dst, p, bytes, cudaMemcpyHostToDevice, g->stream));
+  else return stage_copy(dst, p, bytes, p);
+  return 0;
+}
+
+// How a collective's two buffers lie on this rank.
+enum Layout {
+  kApart,      // separate buffers
+  kSendOnly,   // this rank's recv is not written (Bcast root, Reduce and Gatherv off root)
+  kRecvOnly,   // this rank's send is not read (Bcast and Scatterv off root)
+  kRecvInSend, // in place: recv lies `at` bytes into send
+  kSendInRecv, // in place: send lies `at` bytes into recv
+};
+
+// The heap offsets a collective's kernel reads this rank's send from (`in`) and writes its recv to
+// (`out`), and the caller's recv that finish copies `out` back to when it is staged.
+struct Staging {
+  uint64_t in = 0, out = 0;
+  void* recv = nullptr; // nullptr: nothing to copy back
+  size_t rbytes = 0;
+  int memkind = 0;
+};
+
+// Resolves a call's send side (read by this rank) and recv side (written by this rank) to heap
+// offsets.  A side this rank does not use announces the other side's offset; no peer reads or writes
+// it there.  In place, the inner buffer shares the outer one's staging only when the outer one is
+// the send side, because only the send side's staging is filled from the caller: a send inside a
+// staged recv is staged on its own.
+static int stage(Staging& st, int memkind, const void* send, size_t sbytes, void* recv, size_t rbytes, Layout lay = kApart, size_t at = 0) {
+  Buf in, out;
+  int rc;
+  if (lay == kSendInRecv) {
+    if ((rc = resolve(recv, rbytes, memkind, 1, false, out))) return rc;
+    if (!out.staged) in.off = out.off + at;
+    else if ((rc = resolve(send, sbytes, memkind, 0, true, in))) return rc;
+  } else {
+    if (lay != kRecvOnly && (rc = resolve(send, sbytes, memkind, 0, true, in))) return rc;
+    if (lay == kRecvInSend) out = {in.off + at, in.staged};
+    else if (lay == kSendOnly) out.off = in.off;
+    else if ((rc = resolve(recv, rbytes, memkind, 1, false, out))) return rc;
+    if (lay == kRecvOnly) in.off = out.off;
   }
+  st = {in.off, out.off, out.staged ? recv : nullptr, rbytes, memkind};
   return 0;
 }
 
-static int resolve_out(void* p, size_t bytes, int memkind, int which, Buf& out) {
-  size_t off;
-  if (memkind == B200MPI_DEVICE && g->heap.contains(p, bytes, off)) {
-    out.off = off;
-    out.staged = false;
-    return 0;
+// Ends a call on the collective stream.  A staged recv is copied back after the kernel; a
+// synchronous call first waits and copies only when the status word says the call succeeded, so a
+// mismatched call (B200MPI_ERR_PEER) leaves the caller's buffer untouched, as on the heap.  The
+// _async entries enqueue the copy-back without waiting: they take only DEVICE memory, and
+// b200mpi_stream_sync reports their status (a staged recv of a failed _async call is overwritten).
+static int finish(bool async, const Staging& st = {}) {
+  if (st.recv && st.rbytes) {
+    if (!async) {
+      CUDA_OK(cudaStreamSynchronize(g->stream));
+      const int rc = check_status();
+      if (rc) return rc;
+    }
+    const char* src = (const char*)g->heap.base[g->ctrl.rank] + st.out;
+    if (st.memkind == B200MPI_HOST) CUDA_OK(cudaMemcpyAsync(st.recv, src, st.rbytes, cudaMemcpyDeviceToHost, g->stream));
+    else if (const int rc = stage_copy(st.recv, src, st.rbytes, st.recv)) return rc;
   }
-  int rc = ensure_stage(which, bytes);
-  if (rc) return rc;
-  out.off = g->stage_off[which];
-  out.staged = true;
-  return 0;
-}
-
-static int copy_out(void* p, size_t bytes, int memkind, const Buf& b) {
-  if (!b.staged || bytes == 0) return 0;
-  const char* src = (const char*)g->heap.base[g->ctrl.rank] + b.off;
-  if (memkind == B200MPI_HOST) CUDA_OK(cudaMemcpyAsync(p, src, bytes, cudaMemcpyDeviceToHost, g->stream));
-  else return stage_copy(p, src, bytes, p);
-  return 0;
-}
-
-static int finish(bool async) {
   if (async) return 0;
   CUDA_OK(cudaStreamSynchronize(g->stream));
   return check_status();
@@ -846,11 +837,11 @@ static int local_copy(void* dst, const void* src, size_t bytes, int memkind, boo
   if (dst == src || bytes == 0) return finish(async);
   if (memkind == B200MPI_HOST) {
     // world of one: the value still makes the round trip through the device (no CPU data path)
-    Buf b;
-    int rc = resolve_in(src, bytes, memkind, 0, b);
+    const int rc = ensure_stage(0, bytes);
     if (rc) return rc;
-    rc = copy_out(dst, bytes, memkind, b);
-    if (rc) return rc;
+    char* st = (char*)g->heap.base[g->ctrl.rank] + g->stage_off[0];
+    CUDA_OK(cudaMemcpyAsync(st, src, bytes, cudaMemcpyHostToDevice, g->stream));
+    CUDA_OK(cudaMemcpyAsync(dst, st, bytes, cudaMemcpyDeviceToHost, g->stream));
   } else {
     const bool local = on_this_gpu(dst, bytes) && on_this_gpu(src, bytes);
     int rc = local ? launch_local_copy(dst, src, bytes, g->stream) : launch_copy(dst, src, bytes, g->stream);
@@ -860,13 +851,7 @@ static int local_copy(void* dst, const void* src, size_t bytes, int memkind, boo
 }
 
 // A device-wide rendezvous with nothing in between, on `s`.
-static int launch_barrier(cudaStream_t s) {
-  g->cur_sig = make_sig(3, 0, 0, 0, 0);
-  Comm c = next_comm();
-  sig_grid(c, 1);
-  barrier_kernel<<<1, 32, 0, s>>>(c);
-  return launch_check("barrier_kernel");
-}
+static int launch_barrier(cudaStream_t s) { return launch_coll(barrier_kernel, "barrier_kernel", make_sig(3, 0, 0, 0, 0), 1, 32, 0, s); }
 
 // The LL sequence has crossed 2^32 (ll_seq_next): a lane cell may already hold the value about to be
 // issued, zeros from Init or a value written 2^32 calls ago.  A barrier (no peer is still pushing cells
@@ -1111,14 +1096,29 @@ static int host_pipeline(const PipeSpec& sp) {
   return check_status();
 }
 
-static int do_allreduce(const void* send, void* recv, size_t count, int dtype, int op, int memkind, bool async) {
+// What every collective checks first, in this order: the data plane, the dtype (a reduction refuses
+// u8 and unknown types as unsupported), a reduction's op, a rooted call's root and the memory kind.
+// es receives the element size.  Each call then checks its own NULL-buffer and in-place rules.
+enum { kReduces = 1, kRooted = 2 };
+static int check_coll(const char* what, int traits, int dtype, int op, int root, int memkind, size_t& es) {
   int rc = need_data_plane();
   if (rc) return rc;
-  const size_t es = esize(dtype);
-  if (es == 0 || dtype == B200MPI_U8) return fail(B200MPI_ERR_UNSUPPORTED, "allreduce: dtype must be f32, f64 or i64");
-  if (op < B200MPI_SUM || op > B200MPI_MIN) return fail(B200MPI_ERR_ARG, "allreduce: unknown op");
-  if (count && (!send || !recv)) return fail(B200MPI_ERR_ARG, "allreduce: NULL buffer with count > 0");
-  if (memkind != B200MPI_HOST && memkind != B200MPI_DEVICE) return fail(B200MPI_ERR_ARG, "allreduce: bad memkind");
+  auto arg = [&](const char* msg) { return fail(B200MPI_ERR_ARG, std::string(what) + ": " + msg); };
+  es = esize(dtype);
+  if ((traits & kReduces) && (es == 0 || dtype == B200MPI_U8)) return fail(B200MPI_ERR_UNSUPPORTED, std::string(what) + ": dtype must be f32, f64 or i64");
+  if (es == 0) return arg("unknown dtype");
+  if ((traits & kReduces) && (op < B200MPI_SUM || op > B200MPI_MIN)) return arg("unknown op");
+  if ((traits & kRooted) && (root < 0 || root >= g->ctrl.n)) return arg("root out of range");
+  if (memkind != B200MPI_HOST && memkind != B200MPI_DEVICE) return arg("bad memkind");
+  return 0;
+}
+static int null_buffer(const char* what) { return fail(B200MPI_ERR_ARG, std::string(what) + ": NULL buffer with count > 0"); }
+
+static int do_allreduce(const void* send, void* recv, size_t count, int dtype, int op, int memkind, bool async) {
+  size_t es;
+  int rc = check_coll("allreduce", kReduces, dtype, op, 0, memkind, es);
+  if (rc) return rc;
+  if (count && (!send || !recv)) return null_buffer("allreduce");
   const size_t bytes = count * es;
   if (memkind == B200MPI_HOST && !async && bytes >= g->pipe_min_bytes) {
     PipeSpec sp = {B200MPI_COLL_ALLREDUCE, dtype, op, 0, count, (const char*)send, (char*)recv};
@@ -1134,26 +1134,17 @@ static int do_allreduce(const void* send, void* recv, size_t count, int dtype, i
     }
     return allreduce_ll_host(send, recv, count, dtype, op);
   }
-  Buf in, out;
-  rc = resolve_in(send, bytes, memkind, 0, in);
-  if (rc) return rc;
-  if (send == recv) out = in;
-  else { rc = resolve_out(recv, bytes, memkind, 1, out); if (rc) return rc; }
-  rc = launch_allreduce(algo, dtype, op, in.off, out.off, count, g->stream);
-  if (rc) return rc;
-  rc = copy_out(recv, bytes, memkind, out);
-  if (rc) return rc;
-  return finish(async);
+  Staging st;
+  if ((rc = stage(st, memkind, send, bytes, recv, bytes, send == recv ? kRecvInSend : kApart))) return rc;
+  if ((rc = launch_allreduce(algo, dtype, op, st.in, st.out, count, g->stream))) return rc;
+  return finish(async, st);
 }
 
 static int do_bcast(void* buf, size_t count, int dtype, int root, int memkind, bool async) {
-  int rc = need_data_plane();
+  size_t es;
+  int rc = check_coll("bcast", kRooted, dtype, 0, root, memkind, es);
   if (rc) return rc;
-  const size_t es = esize(dtype);
-  if (es == 0) return fail(B200MPI_ERR_ARG, "bcast: unknown dtype");
-  if (root < 0 || root >= g->ctrl.n) return fail(B200MPI_ERR_ARG, "bcast: root out of range");
-  if (count && !buf) return fail(B200MPI_ERR_ARG, "bcast: NULL buffer with count > 0");
-  if (memkind != B200MPI_HOST && memkind != B200MPI_DEVICE) return fail(B200MPI_ERR_ARG, "bcast: bad memkind");
+  if (count && !buf) return null_buffer("bcast");
   if (g->ctrl.n == 1) return finish(async);
   const size_t bytes = count * es;
   const bool is_root = g->ctrl.rank == root;
@@ -1161,23 +1152,17 @@ static int do_bcast(void* buf, size_t count, int dtype, int root, int memkind, b
     PipeSpec sp = {B200MPI_COLL_BCAST, dtype, 0, root, count, is_root ? (const char*)buf : nullptr, is_root ? nullptr : (char*)buf};
     return host_pipeline(sp);
   }
-  Buf b;
-  if (is_root) rc = resolve_in(buf, bytes, memkind, 0, b);
-  else rc = resolve_out(buf, bytes, memkind, 0, b);
-  if (rc) return rc;
-  rc = launch_bcast(pick_bcast(bytes), dtype, count, b.off, bytes, root, g->stream);
-  if (rc) return rc;
-  if (!is_root) { rc = copy_out(buf, bytes, memkind, b); if (rc) return rc; }
-  return finish(async);
+  Staging st;
+  if ((rc = stage(st, memkind, buf, bytes, buf, bytes, is_root ? kSendOnly : kRecvOnly))) return rc;
+  if ((rc = launch_bcast(pick_bcast(bytes), dtype, count, st.in, bytes, root, g->stream))) return rc;
+  return finish(async, st);
 }
 
 static int do_allgather(const void* send, void* recv, size_t count, int dtype, int memkind, bool async) {
-  int rc = need_data_plane();
+  size_t es;
+  int rc = check_coll("allgather", 0, dtype, 0, 0, memkind, es);
   if (rc) return rc;
-  const size_t es = esize(dtype);
-  if (es == 0) return fail(B200MPI_ERR_ARG, "allgather: unknown dtype");
-  if (count && (!send || !recv)) return fail(B200MPI_ERR_ARG, "allgather: NULL buffer with count > 0");
-  if (memkind != B200MPI_HOST && memkind != B200MPI_DEVICE) return fail(B200MPI_ERR_ARG, "allgather: bad memkind");
+  if (count && (!send || !recv)) return null_buffer("allgather");
   const size_t bytes = count * es;
   const int n = g->ctrl.n;
   if (memkind == B200MPI_HOST && !async && bytes * n >= g->pipe_min_bytes) {
@@ -1185,98 +1170,63 @@ static int do_allgather(const void* send, void* recv, size_t count, int dtype, i
     return host_pipeline(sp);
   }
   if (n == 1) return local_copy(recv, send, bytes, memkind, async);
-  Buf out, in;
-  rc = resolve_out(recv, bytes * n, memkind, 1, out);
-  if (rc) return rc;
-  const bool inplace = (const char*)send == (const char*)recv + (size_t)g->ctrl.rank * bytes;
-  if (inplace && !out.staged) { in.off = out.off + (size_t)g->ctrl.rank * bytes; }
-  else { rc = resolve_in(send, bytes, memkind, 0, in); if (rc) return rc; }
-  rc = launch_allgather(pick_allgather(bytes), dtype, count, in.off, out.off, bytes, g->stream);
-  if (rc) return rc;
-  rc = copy_out(recv, bytes * n, memkind, out);
-  if (rc) return rc;
-  return finish(async);
+  const size_t at = (size_t)g->ctrl.rank * bytes;
+  Staging st;
+  if ((rc = stage(st, memkind, send, bytes, recv, bytes * n, (const char*)send == (const char*)recv + at ? kSendInRecv : kApart, at))) return rc;
+  if ((rc = launch_allgather(pick_allgather(bytes), dtype, count, st.in, st.out, bytes, g->stream))) return rc;
+  return finish(async, st);
 }
 
 // ReduceScatter: send holds size()*count elements (block j is reduced onto rank j), recv holds count.
 static int do_reduce_scatter(const void* send, void* recv, size_t count, int dtype, int op, int memkind, bool async) {
-  int rc = need_data_plane();
+  size_t es;
+  int rc = check_coll("reduce_scatter", kReduces, dtype, op, 0, memkind, es);
   if (rc) return rc;
-  const size_t es = esize(dtype);
-  if (es == 0 || dtype == B200MPI_U8) return fail(B200MPI_ERR_UNSUPPORTED, "reduce_scatter: dtype must be f32, f64 or i64");
-  if (op < B200MPI_SUM || op > B200MPI_MIN) return fail(B200MPI_ERR_ARG, "reduce_scatter: unknown op");
-  if (count && (!send || !recv)) return fail(B200MPI_ERR_ARG, "reduce_scatter: NULL buffer with count > 0");
-  if (memkind != B200MPI_HOST && memkind != B200MPI_DEVICE) return fail(B200MPI_ERR_ARG, "reduce_scatter: bad memkind");
+  if (count && (!send || !recv)) return null_buffer("reduce_scatter");
   const size_t bytes = count * es;
   const int n = g->ctrl.n;
   if (n == 1) return local_copy(recv, send, bytes, memkind, async);
-  Buf in, out;
-  rc = resolve_in(send, bytes * n, memkind, 0, in);
-  if (rc) return rc;
-  const bool inplace = (const char*)recv == (const char*)send + (size_t)g->ctrl.rank * bytes;
-  if (inplace) { out.off = in.off + (size_t)g->ctrl.rank * bytes; out.staged = in.staged; }
-  else { rc = resolve_out(recv, bytes, memkind, 1, out); if (rc) return rc; }
-  rc = launch_reduce_scatter(pick_reduce_scatter(bytes, dtype, op), dtype, op, in.off, out.off, count, g->stream);
-  if (rc) return rc;
-  rc = copy_out(recv, bytes, memkind, out);
-  if (rc) return rc;
-  return finish(async);
+  const size_t at = (size_t)g->ctrl.rank * bytes;
+  Staging st;
+  if ((rc = stage(st, memkind, send, bytes * n, recv, bytes, (const char*)recv == (const char*)send + at ? kRecvInSend : kApart, at))) return rc;
+  if ((rc = launch_reduce_scatter(pick_reduce_scatter(bytes, dtype, op), dtype, op, st.in, st.out, count, g->stream))) return rc;
+  return finish(async, st);
 }
 
 // Reduce: like Allreduce but only `root`'s recv is written (recv may be NULL elsewhere).
 static int do_reduce(const void* send, void* recv, size_t count, int dtype, int op, int root, int memkind, bool async) {
-  int rc = need_data_plane();
+  size_t es;
+  int rc = check_coll("reduce", kReduces | kRooted, dtype, op, root, memkind, es);
   if (rc) return rc;
-  const size_t es = esize(dtype);
   const int n = g->ctrl.n;
-  if (es == 0 || dtype == B200MPI_U8) return fail(B200MPI_ERR_UNSUPPORTED, "reduce: dtype must be f32, f64 or i64");
-  if (op < B200MPI_SUM || op > B200MPI_MIN) return fail(B200MPI_ERR_ARG, "reduce: unknown op");
-  if (root < 0 || root >= n) return fail(B200MPI_ERR_ARG, "reduce: root out of range");
   const bool is_root = g->ctrl.rank == root;
-  if (count && (!send || (is_root && !recv))) return fail(B200MPI_ERR_ARG, "reduce: NULL buffer with count > 0");
-  if (memkind != B200MPI_HOST && memkind != B200MPI_DEVICE) return fail(B200MPI_ERR_ARG, "reduce: bad memkind");
+  if (count && (!send || (is_root && !recv))) return null_buffer("reduce");
   const size_t bytes = count * es;
   if (n == 1) return local_copy(recv, send, bytes, memkind, async);
-  Buf in, out;
-  rc = resolve_in(send, bytes, memkind, 0, in);
-  if (rc) return rc;
-  out = in; // non-roots announce their send offset as recv offset; nobody writes there
-  if (is_root && recv != send) { rc = resolve_out(recv, bytes, memkind, 1, out); if (rc) return rc; }
+  Staging st;
+  if ((rc = stage(st, memkind, send, bytes, recv, bytes, !is_root ? kSendOnly : recv == send ? kRecvInSend : kApart))) return rc;
   int algo = g->algo[B200MPI_COLL_ALLREDUCE] == B200MPI_ALGO_TWOSHOT ? B200MPI_ALGO_TWOSHOT
              : (g->heap.mc_base && nvls_supports(dtype, op) && n >= g->nvls_min_ranks) ? B200MPI_ALGO_NVLS : B200MPI_ALGO_TWOSHOT;
-  rc = launch_reduce(algo, dtype, op, in.off, out.off, count, root, g->stream);
-  if (rc) return rc;
-  if (is_root) { rc = copy_out(recv, bytes, memkind, out); if (rc) return rc; }
-  return finish(async);
+  if ((rc = launch_reduce(algo, dtype, op, st.in, st.out, count, root, g->stream))) return rc;
+  return finish(async, st);
 }
 
 // Alltoall: send and recv hold size()*count elements; block j of send goes to rank j's block rank().
 static int do_alltoall(const void* send, void* recv, size_t count, int dtype, int memkind, bool async) {
-  int rc = need_data_plane();
+  size_t es;
+  int rc = check_coll("alltoall", 0, dtype, 0, 0, memkind, es);
   if (rc) return rc;
-  const size_t es = esize(dtype);
-  if (es == 0) return fail(B200MPI_ERR_ARG, "alltoall: unknown dtype");
-  if (count && (!send || !recv)) return fail(B200MPI_ERR_ARG, "alltoall: NULL buffer with count > 0");
+  if (count && (!send || !recv)) return null_buffer("alltoall");
   if (send == recv && count) return fail(B200MPI_ERR_ARG, "alltoall: in place is not supported");
-  if (memkind != B200MPI_HOST && memkind != B200MPI_DEVICE) return fail(B200MPI_ERR_ARG, "alltoall: bad memkind");
   const size_t bytes = count * es;
   const int n = g->ctrl.n;
   if (n == 1) return local_copy(recv, send, bytes, memkind, async);
-  Buf in, out;
-  rc = resolve_in(send, bytes * n, memkind, 0, in);
-  if (rc) return rc;
-  rc = resolve_out(recv, bytes * n, memkind, 1, out);
-  if (rc) return rc;
-  g->cur_sig = make_sig(6, dtype, 0, 0, count);
-  Comm c = next_comm();
+  Staging st;
+  if ((rc = stage(st, memkind, send, bytes * n, recv, bytes * n))) return rc;
+  const uint64_t sig = make_sig(6, dtype, 0, 0, count);
   const int blocks = grid_for(bytes / 16 + 1, 4);
-  sig_grid(c, blocks);
-  with_unit(in.off | out.off | bytes, [&](auto u) { alltoall_kernel<decltype(u), 4><<<blocks, kThreads, 0, g->stream>>>(c, in.off, out.off, bytes); });
-  rc = launch_check("alltoall_kernel");
-  if (rc) return rc;
-  rc = copy_out(recv, bytes * n, memkind, out);
-  if (rc) return rc;
-  return finish(async);
+  rc = with_unit(st.in | st.out | bytes, [&](auto u) { return launch_coll(alltoall_kernel<decltype(u), 4>, "alltoall_kernel", sig, blocks, kThreads, 0, g->stream, st.in, st.out, bytes); });
+  return rc ? rc : finish(async, st);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1314,93 +1264,55 @@ static uint64_t vtable_bits(const VTable& vt) {
   return m;
 }
 
-// A staged result is copied back only after the collective succeeded: a mismatched call
-// (B200MPI_ERR_PEER) leaves the caller's buffer untouched, as it does for heap buffers.
-static int copy_out_checked(void* p, size_t bytes, int memkind, const Buf& b) {
-  if (!b.staged || bytes == 0) return 0;
-  CUDA_OK(cudaStreamSynchronize(g->stream));
-  int rc = check_status();
-  if (rc) return rc;
-  return copy_out(p, bytes, memkind, b);
-}
-
-static int check_v_args(const char* what, int dtype, int memkind, size_t& es) {
-  es = esize(dtype);
-  if (es == 0) return fail(B200MPI_ERR_ARG, std::string(what) + ": unknown dtype");
-  if (memkind != B200MPI_HOST && memkind != B200MPI_DEVICE) return fail(B200MPI_ERR_ARG, std::string(what) + ": bad memkind");
-  return 0;
-}
-
 // Gatherv: rank r's send lands at displacement r of root's recv; recv may be NULL off root.
 // Allgatherv (all): it lands at displacement r of every rank's recv.
 static int do_gatherv(const void* send, void* recv, const size_t* counts, int dtype, int root, bool all, int memkind) {
-  int rc = need_data_plane();
-  if (rc) return rc;
   const char* what = all ? "allgatherv" : "gatherv";
-  const int n = g->ctrl.n, me = g->ctrl.rank;
   size_t es;
-  if ((rc = check_v_args(what, dtype, memkind, es))) return rc;
+  int rc = check_coll(what, all ? 0 : kRooted, dtype, 0, root, memkind, es);
+  if (rc) return rc;
   if (all) root = -1;
-  else if (root < 0 || root >= n) return fail(B200MPI_ERR_ARG, "gatherv: root out of range");
+  const int n = g->ctrl.n, me = g->ctrl.rank;
   VTable vt;
   uint64_t hash;
   if ((rc = make_vtable(what, counts, es, vt, hash))) return rc;
   const size_t mine = vt.off[me + 1] - vt.off[me], total = vt.off[n];
   const bool gets = all || me == root; // this rank's recv is written
-  if ((mine && !send) || (gets && total && !recv)) return fail(B200MPI_ERR_ARG, std::string(what) + ": NULL buffer with count > 0");
-  const bool inplace = gets && recv && (const char*)send == (const char*)recv + vt.off[me];
+  if ((mine && !send) || (gets && total && !recv)) return null_buffer(what);
   if (n == 1) return local_copy(recv, send, total, memkind, false);
-  Buf in, out;
-  if (gets) {
-    rc = resolve_out(recv, total, memkind, 1, out);
-    if (rc) return rc;
-  }
-  if (inplace && !out.staged) in.off = out.off + vt.off[me];
-  else if ((rc = resolve_in(send, mine, memkind, 0, in))) return rc;
-  if (!gets) out = in; // announced but never written: only root's recv is a destination
-  g->cur_sig = make_sig(all ? 9 : 7, dtype, root, 0, total / es, hash);
-  Comm c = next_comm();
+  const bool inplace = gets && recv && (const char*)send == (const char*)recv + vt.off[me];
+  Staging st; // off root the recv is announced but never written: only root's recv is a destination
+  if ((rc = stage(st, memkind, send, mine, recv, total, !gets ? kSendOnly : inplace ? kSendInRecv : kApart, vt.off[me]))) return rc;
+  const uint64_t sig = make_sig(all ? 9 : 7, dtype, root, 0, total / es, hash);
   const int blocks = vtable_grid(vt);
-  sig_grid(c, blocks);
-  with_unit(in.off | out.off | vtable_bits(vt), [&](auto u) { gatherv_push_kernel<decltype(u), 4><<<blocks, kThreads, 0, g->stream>>>(c, in.off, out.off, vt, root); });
-  if ((rc = launch_check("gatherv_push_kernel"))) return rc;
-  if (gets && (rc = copy_out_checked(recv, total, memkind, out))) return rc;
-  return finish(false);
+  rc = with_unit(st.in | st.out | vtable_bits(vt), [&](auto u) {
+    return launch_coll(gatherv_push_kernel<decltype(u), 4>, "gatherv_push_kernel", sig, blocks, kThreads, 0, g->stream, st.in, st.out, vt, root);
+  });
+  return rc ? rc : finish(false, st);
 }
 
 // Scatterv: block r of root's send (NULL allowed off root) goes to rank r's recv.
 static int do_scatterv(const void* send, void* recv, const size_t* counts, int dtype, int root, int memkind) {
-  int rc = need_data_plane();
+  size_t es;
+  int rc = check_coll("scatterv", kRooted, dtype, 0, root, memkind, es);
   if (rc) return rc;
   const int n = g->ctrl.n, me = g->ctrl.rank;
-  size_t es;
-  if ((rc = check_v_args("scatterv", dtype, memkind, es))) return rc;
-  if (root < 0 || root >= n) return fail(B200MPI_ERR_ARG, "scatterv: root out of range");
   VTable vt;
   uint64_t hash;
   if ((rc = make_vtable("scatterv", counts, es, vt, hash))) return rc;
   const size_t mine = vt.off[me + 1] - vt.off[me], total = vt.off[n];
   const bool is_root = me == root;
-  if ((mine && !recv) || (is_root && total && !send)) return fail(B200MPI_ERR_ARG, "scatterv: NULL buffer with count > 0");
+  if ((mine && !recv) || (is_root && total && !send)) return null_buffer("scatterv");
   if (n == 1) return local_copy(recv, send, total, memkind, false);
-  Buf in, out;
-  if (is_root) {
-    rc = resolve_in(send, total, memkind, 0, in);
-    if (rc) return rc;
-  }
   const bool inplace = is_root && send && (const char*)recv == (const char*)send + vt.off[me];
-  if (inplace && !in.staged) out.off = in.off + vt.off[me];
-  else if ((rc = resolve_out(recv, mine, memkind, 1, out))) return rc;
-  if (!is_root) in = out; // announced but never read: only root's send is a source
-  g->cur_sig = make_sig(8, dtype, root, 0, total / es, hash);
-  Comm c = next_comm();
+  Staging st; // off root the send is announced but never read: only root's send is a source
+  if ((rc = stage(st, memkind, send, total, recv, mine, !is_root ? kRecvOnly : inplace ? kRecvInSend : kApart, vt.off[me]))) return rc;
+  const uint64_t sig = make_sig(8, dtype, root, 0, total / es, hash);
   const int blocks = vtable_grid(vt);
-  sig_grid(c, blocks);
-  with_unit(in.off | out.off | vtable_bits(vt), [&](auto u) { scatterv_pull_kernel<decltype(u), 4><<<blocks, kThreads, 0, g->stream>>>(c, in.off, out.off, vt, root); });
-  if ((rc = launch_check("scatterv_pull_kernel"))) return rc;
-  rc = copy_out_checked(recv, mine, memkind, out);
-  if (rc) return rc;
-  return finish(false);
+  rc = with_unit(st.in | st.out | vtable_bits(vt), [&](auto u) {
+    return launch_coll(scatterv_pull_kernel<decltype(u), 4>, "scatterv_pull_kernel", sig, blocks, kThreads, 0, g->stream, st.in, st.out, vt, root);
+  });
+  return rc ? rc : finish(false, st);
 }
 
 // The fixed-count forms: the uniform table.
@@ -1416,39 +1328,37 @@ static int do_gather(const void* send, void* recv, size_t count, int dtype, int 
 // holds a different table, so the tables are checked on the device (sync_start_pairs) and a
 // mismatch ends as B200MPI_ERR_PEER on every rank with no buffer touched.
 static int do_alltoallv(const void* send, const size_t* send_counts, void* recv, const size_t* recv_counts, int dtype, int memkind) {
-  int rc = need_data_plane();
+  size_t es;
+  int rc = check_coll("alltoallv", 0, dtype, 0, 0, memkind, es);
   if (rc) return rc;
   const int n = g->ctrl.n, me = g->ctrl.rank;
-  size_t es;
-  if ((rc = check_v_args("alltoallv", dtype, memkind, es))) return rc;
   if (!send_counts || !recv_counts) return fail(B200MPI_ERR_ARG, "alltoallv: NULL counts table");
   VTable sv, rv;
   uint64_t digest;
   if (!a2av_tables(me, n, send_counts, recv_counts, es, sv, rv, digest)) return fail(B200MPI_ERR_ARG, "alltoallv: sum(counts) * element size overflows");
   const size_t sbytes = sv.off[n], rbytes = rv.off[n];
-  if ((sbytes && !send) || (rbytes && !recv)) return fail(B200MPI_ERR_ARG, "alltoallv: NULL buffer with count > 0");
+  if ((sbytes && !send) || (rbytes && !recv)) return null_buffer("alltoallv");
   if (send == recv && (sbytes || rbytes)) return fail(B200MPI_ERR_ARG, "alltoallv: in place is not supported");
   if (n == 1) {
     if (send_counts[0] != recv_counts[0]) return fail(B200MPI_ERR_PEER, "alltoallv: send_counts[0] != recv_counts[0] in a world of one; buffers were left untouched");
     return local_copy(recv, send, sbytes, memkind, false);
   }
-  Buf in, out;
-  if ((rc = resolve_in(send, sbytes, memkind, 0, in))) return rc;
-  if ((rc = resolve_out(recv, rbytes, memkind, 1, out))) return rc;
-  g->cur_sig = make_sig(10, dtype, 0, 0, 0);
+  Staging st;
+  if ((rc = stage(st, memkind, send, sbytes, recv, rbytes))) return rc;
   // The grid is block_cap() CTAs whatever the table: the barriers pair CTAs by blockIdx and the grid
   // is part of the signature, so it may depend only on what every rank shares.  The access unit
-  // follows this rank's offsets and both of its displacement tables.
-  Comm c = next_comm();
+  // follows this rank's offsets and both of its displacement tables.  The table digest goes into the
+  // signature this rank announces after the grid (sync_start_pairs), so this launch is its own.
   const int blocks = block_cap();
+  Comm c = next_comm(make_sig(10, dtype, 0, 0, 0));
   sig_grid(c, blocks);
   const uint64_t base_sig = c.sig;
   c.sig = base_sig + digest;
-  with_unit(in.off | out.off | vtable_bits(sv) | vtable_bits(rv),
-            [&](auto u) { alltoallv_push_kernel<decltype(u), 4><<<blocks, kThreads, 0, g->stream>>>(c, in.off, out.off, sv, rv, base_sig); });
-  if ((rc = launch_check("alltoallv_push_kernel"))) return rc;
-  if ((rc = copy_out_checked(recv, rbytes, memkind, out))) return rc;
-  return finish(false);
+  rc = with_unit(st.in | st.out | vtable_bits(sv) | vtable_bits(rv), [&](auto u) {
+    alltoallv_push_kernel<decltype(u), 4><<<blocks, kThreads, 0, g->stream>>>(c, st.in, st.out, sv, rv, base_sig);
+    return launch_check("alltoallv_push_kernel");
+  });
+  return rc ? rc : finish(false, st);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -825,6 +825,33 @@ def scenario_mismatch(a):
         rc = lib.b200mpi_allgather(x.ptr, y.ptr, 1000 // n, L.F32, L.DEVICE)
     assert rc == L.ERR_PEER, (rc, L.last_error())
     done += 1
+    # Host slices go through a staging block.  A successful call of the same size first leaves its
+    # result there; the mismatched call must not copy that back.  ll_max_bytes = 0 keeps Allreduce on
+    # a signed path (the LL kernel carries no signature).
+    old_ll = L.get_param("ll_max_bytes")
+    assert lib.b200mpi_set_param(b"ll_max_bytes", 0) == 0
+    c, root = 1000, n - 1
+    assert c * n * 4 < L.get_param("pipe_min_bytes")
+    calls = (  # name, send and recv elements, call(send, recv, count); Bcast reads on root and writes elsewhere
+        ("allreduce", c, c, lambda s, r, k: lib.b200mpi_allreduce(s, r, k, L.F32, L.SUM, L.HOST)),
+        ("bcast", c, c, lambda s, r, k: lib.b200mpi_bcast(s if rank == 0 else r, k, L.F32, 0, L.HOST)),
+        ("allgather", c, c * n, lambda s, r, k: lib.b200mpi_allgather(s, r, k, L.F32, L.HOST)),
+        ("reduce_scatter", c * n, c, lambda s, r, k: lib.b200mpi_reduce_scatter(s, r, k, L.F32, L.SUM, L.HOST)),
+        ("reduce", c, c, lambda s, r, k: lib.b200mpi_reduce(s, r, k, L.F32, L.SUM, root, L.HOST)),
+        ("alltoall", c * n, c * n, lambda s, r, k: lib.b200mpi_alltoall(s, r, k, L.F32, L.HOST)),
+    )
+    for name, ns, nr, call in calls:
+        send = np.arange(ns, dtype=np.float32) + 10 * (rank + 1)
+        recv = np.full(nr, -5, dtype=np.float32)
+        rc = call(send.ctypes.data, recv.ctypes.data, c)
+        assert rc == 0, (name, rc, L.last_error())
+        recv[:] = -5
+        rc = call(send.ctypes.data, recv.ctypes.data, c if rank == 0 else c - 1)
+        assert rc == L.ERR_PEER, (name, rc, L.last_error())
+        check_equal(recv, np.full(nr, -5, dtype=np.float32), "%s: host recv untouched after a mismatched call" % name)
+        check_equal(send, np.arange(ns, dtype=np.float32) + 10 * (rank + 1), "%s: host send untouched after a mismatched call" % name)
+        done += 1
+    assert lib.b200mpi_set_param(b"ll_max_bytes", old_ll) == 0
     # and the world still works
     mpi.Allreduce(x, y)
     check_equal(y.to_host(), np.full(1000, n, dtype=np.float32), "allreduce after mismatches")

@@ -352,6 +352,42 @@ func (c *Cuda) Reduce(send, recv interface{}, op Op, root int) error {
 	return nil
 }
 
+// scan lowers Scan and Exscan; Exscan's recv may be nil on rank 0, where it is not written.
+func (c *Cuda) scan(what string, send, recv interface{}, op Op) error {
+	sp, sn, sdt, sk, err := lowerTyped(what, send)
+	if err != nil {
+		return err
+	}
+	var rp unsafe.Pointer
+	if recv != nil {
+		var rn int
+		var rdt, rk C.int
+		rp, rn, rdt, rk, err = lowerTyped(what, recv)
+		if err != nil {
+			return err
+		}
+		if sn != rn || sdt != rdt || sk != rk {
+			return fmt.Errorf("mpi: %s send and recv must have the same type, length and memory kind", what)
+		}
+	}
+	var rc C.int
+	if what == "Scan" {
+		rc = C.b200mpi_scan(sp, rp, C.size_t(sn), sdt, C.int(op), sk)
+	} else {
+		rc = C.b200mpi_exscan(sp, rp, C.size_t(sn), sdt, C.int(op), sk)
+	}
+	if rc != 0 {
+		return lastError(rc, 0)
+	}
+	return nil
+}
+
+// Scan: rank r's recv = send_0 op ... op send_r, combined in rank order.
+func (c *Cuda) Scan(send, recv interface{}, op Op) error { return c.scan("Scan", send, recv, op) }
+
+// Exscan: rank r's recv = send_0 op ... op send_{r-1}; rank 0's recv is not written.
+func (c *Cuda) Exscan(send, recv interface{}, op Op) error { return c.scan("Exscan", send, recv, op) }
+
 // Alltoall: block j of send becomes block Rank() of rank j's recv.
 func (c *Cuda) Alltoall(send, recv interface{}) error {
 	sp, sn, sdt, sk, err := lowerTyped("Alltoall", send)

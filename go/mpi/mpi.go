@@ -27,6 +27,7 @@
 //	Gather, Scatter                   rooted collection and distribution of equal blocks
 //	Gatherv, Scatterv, Allgatherv     the same with a different length on every rank
 //	Alltoallv                         Alltoall with a different length for every (source, destination) pair
+//	Scan, Exscan                      prefix reductions in rank order (inclusive, exclusive)
 //	Isend + Wait   the non-blocking Send design the reference sketches and comments out (mpi.go:132-152)
 //
 // They are served through the optional Collective interface, the upgrade the reference hints at
@@ -87,6 +88,12 @@ type Collective3 interface {
 // tables, sendCounts and recvCounts are this rank's own row and column and differ from rank to rank.
 type Collective4 interface {
 	Alltoallv(send interface{}, sendCounts []int, recv interface{}, recvCounts []int) ([]int, error)
+}
+
+// Collective5 is the fifth optional upgrade: the prefix reductions.
+type Collective5 interface {
+	Scan(send, recv interface{}, op Op) error
+	Exscan(send, recv interface{}, op Op) error
 }
 
 // Raw marks a payload that is sent as bytes without any encoding.
@@ -318,4 +325,32 @@ func Alltoallv(send interface{}, sendCounts []int, recv interface{}, recvCounts 
 		return nil, fmt.Errorf("mpi: registered implementation %T has no Alltoallv", current)
 	}
 	return c.Alltoallv(send, sendCounts, recv, recvCounts)
+}
+
+func collective5(what string) (Collective5, error) {
+	if c, ok := current.(Collective5); ok {
+		return c, nil
+	}
+	return nil, fmt.Errorf("mpi: registered implementation %T has no %s", current, what)
+}
+
+// Scan stores send_0 op send_1 op ... op send_r, combined in rank order, in rank r's recv. send and
+// recv are slices of the same type and length ([]float32, []float64, []int64) and may be the same slice.
+func Scan(send, recv interface{}, op Op) error {
+	c, err := collective5("Scan")
+	if err != nil {
+		return err
+	}
+	return c.Scan(send, recv, op)
+}
+
+// Exscan is Scan without rank r's own send: rank r >= 1 receives send_0 op ... op send_{r-1}.
+// Rank 0's recv is not written and may be nil. An Exscan of each rank's element count gives its
+// offset in a buffer packed in rank order.
+func Exscan(send, recv interface{}, op Op) error {
+	c, err := collective5("Exscan")
+	if err != nil {
+		return err
+	}
+	return c.Exscan(send, recv, op)
 }

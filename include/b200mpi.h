@@ -31,7 +31,8 @@ extern "C" {
 #endif
 
 #define B200MPI_VERSION 200 /* 0.2.0: + isend/wait, reduce_scatter, reduce, alltoall, probes, get_param;
-                               then gather, scatter, gatherv, scatterv, allgatherv, alltoallv (all additive) */
+                               then gather, scatter, gatherv, scatterv, allgatherv, alltoallv, scan, exscan
+                               (all additive) */
 #define B200MPI_MAX_RANKS 8 /* "the 8 GPUs of one box" */
 
 typedef enum {
@@ -169,6 +170,13 @@ int b200mpi_allgatherv(const void* send, void* recv, const size_t* counts, int d
  * the b200mpi_alloc heap are staged whole through it (B200MPI_ERR_NOMEM if too big). */
 int b200mpi_alltoallv(const void* send, const size_t* send_counts, void* recv, const size_t* recv_counts,
                       int dtype, int memkind);
+/* Inclusive prefix reduction: recv on rank r = send_0 op send_1 op ... op send_r, element-wise,
+ * combined left to right in rank order.  send == recv is in place. */
+int b200mpi_scan(const void* send, void* recv, size_t count, int dtype, int op, int memkind);
+/* Exclusive: recv on rank r >= 1 = send_0 op ... op send_{r-1}.  Rank 0's recv is not written
+ * (it may be NULL there; in place, rank 0 keeps its input).  For both, buffers outside the
+ * b200mpi_alloc heap are staged whole through it (B200MPI_ERR_NOMEM if too big). */
+int b200mpi_exscan(const void* send, void* recv, size_t count, int dtype, int op, int memkind);
 int b200mpi_barrier(void);
 
 /* Enqueue-only forms on the library stream (DEVICE memkind only). */

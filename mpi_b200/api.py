@@ -6,6 +6,7 @@ Same names, same argument meaning, same blocking behaviour:
     Register(impl)  Interface  Raw  TagExists                       (the reference's surface)
     Recv  Bcast(data, root)  Allreduce(send, recv, op)  Allgather(send, recv)  Barrier()   (new)
     ReduceScatter(send, recv, op)  Reduce(send, recv, op, root)  Alltoall(send, recv)      (new)
+    Scan(send, recv, op)  Exscan(send, recv, op)                                             (new)
     Gather(send, recv, root)  Scatter(send, recv, root)                                       (new)
     Gatherv(send, recv, root, counts)  Scatterv(send, recv, counts, root)  Allgatherv(send, recv, counts)
     Alltoallv(send, send_counts, recv, recv_counts)                                          (new)
@@ -305,6 +306,27 @@ class Cuda(Interface):
         _check(L.load().b200mpi_alltoall(sp, rp, sc // n, sdt, sk))
         return recv
 
+    def Scan(self, send, recv, op=SUM):
+        """Rank r's recv = send_0 op ... op send_r, combined in rank order.  recv is send: in place."""
+        sp, sc, sdt, sk, _, _ = _describe(send)
+        rp, rc_, rdt, rk, _, _ = _describe(recv)
+        if sc != rc_ or sdt != rdt or sk != rk:
+            raise ValueError("mpi: Scan send and recv must have the same length, type and memory kind")
+        _check(L.load().b200mpi_scan(sp, rp, sc, sdt, int(op), sk))
+        return recv
+
+    def Exscan(self, send, recv, op=SUM):
+        """Rank r's recv = send_0 op ... op send_{r-1}; rank 0's recv is not written and may be None
+        there (the library refuses None elsewhere)."""
+        sp, sc, sdt, sk, _, _ = _describe(send)
+        rp = None
+        if recv is not None:
+            rp, rc_, rdt, rk, _, _ = _describe(recv)
+            if sc != rc_ or sdt != rdt or sk != rk:
+                raise ValueError("mpi: Exscan send and recv must have the same length, type and memory kind")
+        _check(L.load().b200mpi_exscan(sp, rp, sc, sdt, int(op), sk))
+        return recv
+
     def Barrier(self):
         _check(L.load().b200mpi_barrier())
 
@@ -536,6 +558,14 @@ def Reduce(send, recv, op=SUM, root=0):
 
 def Alltoall(send, recv):
     return _collective("Alltoall")(send, recv)
+
+
+def Scan(send, recv, op=SUM):
+    return _collective("Scan")(send, recv, op)
+
+
+def Exscan(send, recv, op=SUM):
+    return _collective("Exscan")(send, recv, op)
 
 
 def Gather(send, recv, root):

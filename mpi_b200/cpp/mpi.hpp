@@ -14,7 +14,7 @@
 //   mpi.Register(impl)                         void mpi::Register(Interface*)  (second call throws = panics, mpi.go:61-67)
 //   flag.Parse() + mpi.Flag*                   mpi::ParseFlags(argc, argv) + mpi::Flag*
 //   new: Recv, Bcast, Allreduce, Allgather, Barrier, ReduceScatter, Reduce, Alltoall, Isend/Wait,
-//        Gather, Scatter, Gatherv, Scatterv, Allgatherv, Alltoallv;
+//        Gather, Scatter, Gatherv, Scatterv, Allgatherv, Alltoallv, Scan, Exscan;
 //        mpi::DeviceSlice<T> for heap-resident buffers
 // `data` may be std::vector<double|float|int64_t|uint8_t>, std::string (sent as bytes, the
 // "anything else is gob-encoded" path), or DeviceSlice<T>.
@@ -175,6 +175,9 @@ struct Interface {
   virtual Error ReduceScatter(Buffer, Buffer, Op) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no ReduceScatter"; return e; }
   virtual Error Reduce(Buffer, Buffer, Op, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Reduce"; return e; }
   virtual Error Alltoall(Buffer, Buffer) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Alltoall"; return e; }
+  // prefix reductions in rank order; Exscan leaves rank 0's recv unwritten (it may be empty there)
+  virtual Error Scan(Buffer, Buffer, Op) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Scan"; return e; }
+  virtual Error Exscan(Buffer, Buffer, Op) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Exscan"; return e; }
   // rooted and variable-count collectives: counts[Size()] is the same table on every rank
   virtual Error Gather(Buffer, Buffer, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Gather"; return e; }
   virtual Error Scatter(Buffer, Buffer, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Scatter"; return e; }
@@ -217,6 +220,8 @@ struct Cuda : Interface {
   Error ReduceScatter(Buffer s, Buffer r, Op op) override { return make_error(b200mpi_reduce_scatter(s.ptr, r.ptr, r.count, s.dtype, op, s.memkind)); }
   Error Reduce(Buffer s, Buffer r, Op op, int root) override { return make_error(b200mpi_reduce(s.ptr, r.ptr, s.count, s.dtype, op, root, s.memkind)); }
   Error Alltoall(Buffer s, Buffer r) override { return make_error(b200mpi_alltoall(s.ptr, r.ptr, s.count / (size_t)(Size() > 0 ? Size() : 1), s.dtype, s.memkind)); }
+  Error Scan(Buffer s, Buffer r, Op op) override { return make_error(b200mpi_scan(s.ptr, r.ptr, s.count, s.dtype, op, s.memkind)); }
+  Error Exscan(Buffer s, Buffer r, Op op) override { return make_error(b200mpi_exscan(s.ptr, r.ptr, s.count, s.dtype, op, s.memkind)); }
   Error Gather(Buffer s, Buffer r, int root) override { return make_error(b200mpi_gather(s.ptr, r.ptr, s.count, s.dtype, root, s.memkind)); }
   Error Scatter(Buffer s, Buffer r, int root) override { return make_error(b200mpi_scatter(s.ptr, r.ptr, r.count, r.dtype, root, r.memkind)); }
   Error Gatherv(Buffer s, Buffer r, const size_t* counts, int root) override { return make_error(b200mpi_gatherv(s.ptr, r.ptr, counts, s.dtype, root, s.memkind)); }
@@ -302,6 +307,19 @@ template <typename T> inline Error Alltoall(const std::vector<T>& send, std::vec
   recv->resize(send.size());
   return mpier()->Alltoall(lower(send), lower(*recv));
 }
+
+// Scan: rank r's recv = send_0 op ... op send_r (rank order).  Exscan: up to send_{r-1}; rank 0's
+// recv is not written.  A vector recv is resized to len(send).
+template <typename T> inline Error Scan(const std::vector<T>& send, std::vector<T>* recv, Op op = SUM) {
+  recv->resize(send.size());
+  return mpier()->Scan(lower(send), lower(*recv), op);
+}
+template <typename T> inline Error Scan(const DeviceSlice<T>& send, DeviceSlice<T>* recv, Op op = SUM) { return mpier()->Scan(lower(send), lower(*recv), op); }
+template <typename T> inline Error Exscan(const std::vector<T>& send, std::vector<T>* recv, Op op = SUM) {
+  recv->resize(send.size());
+  return mpier()->Exscan(lower(send), lower(*recv), op);
+}
+template <typename T> inline Error Exscan(const DeviceSlice<T>& send, DeviceSlice<T>* recv, Op op = SUM) { return mpier()->Exscan(lower(send), lower(*recv), op); }
 
 // Gather: root's recv is resized to Size() blocks of len(send).  Scatter: root's recv is resized to
 // one block of send; elsewhere recv must already hold that block length.

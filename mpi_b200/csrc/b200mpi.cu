@@ -319,7 +319,7 @@ static int check_status() {
 // call.  coll: 0 allreduce, 1 bcast, 2 allgather, 3 barrier, 4 reduce_scatter, 5 reduce, 6 alltoall,
 // 7 gather(v), 8 scatter(v), 9 allgatherv (these three carry a hash of the counts table in `total`),
 // 10 alltoallv (whose ranks hold different tables: each adds its table digest to the signature it
-// announces, see sync_start_pairs in kernels.cuh).
+// announces, see sync_start_pairs in kernels.cuh), 11 scan, 12 exscan.
 // `total` is the element count of the whole user call when the launch is one chunk of a pipelined
 // host-slice call (ranks that disagree about the total then disagree from the first chunk on).
 static uint64_t make_sig(int coll, int dtype, int extra, int algo, size_t count, size_t total = 0) {
@@ -607,6 +607,32 @@ static int launch_reduce_scatter(int algo, int dtype, int op, uint64_t so, uint6
         const bool known_dtype = dtype == B200MPI_F32 || dtype == B200MPI_F64 || dtype == B200MPI_I64;
         return known_dtype ? fail(B200MPI_ERR_ARG, "reduce_scatter: unknown op") : fail(B200MPI_ERR_UNSUPPORTED, "reduce_scatter: dtype must be f32, f64 or i64");
       });
+}
+
+// Scan / Exscan: one algorithm, the two-shot ownership and grid.  UNROLL per (n, element size) is
+// the largest for which ptxas reports no spill in any instance.
+static int launch_scan(bool exclusive, int dtype, int op, uint64_t so, uint64_t ro, size_t count, cudaStream_t s) {
+  const uint64_t sig = make_sig(exclusive ? 12 : 11, dtype, op, 0, count);
+  return with_reduction(
+      dtype, op,
+      [&](auto t, auto o) {
+        using T = decltype(t);
+        using Op = decltype(o);
+        const int n = g->ctrl.n;
+        constexpr int EPV = 16 / sizeof(T);
+        const size_t nvec = (count + EPV - 1) / EPV;
+        const size_t per = (nvec + n - 1) / n;
+        const uint32_t sh = own_shift(nvec, n, 0);
+        auto go = [&](auto kernel, int unroll) { return launch_coll(kernel, "scan_kernel", sig, grid_for(per, unroll), kThreads, 0, s, so, ro, count, sh); };
+#define B200_SCAN(NRV, UV) \
+  return exclusive ? go(scan_kernel<T, Op, NRV, UV, true>, UV) : go(scan_kernel<T, Op, NRV, UV, false>, UV);
+        if (n == 2) B200_SCAN(2, (sizeof(T) == 4 ? 8 : 4))
+        else if (n == 4) B200_SCAN(4, 4)
+        else if (n == 8) B200_SCAN(8, 2)
+        else B200_SCAN(0, 1)
+#undef B200_SCAN
+      },
+      [&] { return fail(B200MPI_ERR_UNSUPPORTED, "scan: unsupported dtype/op (need f32, f64 or i64 with sum/max/min)"); });
 }
 
 // AUTO for Allreduce: best busbw / latency per (n, size) among the variants.  The multi-GPU thresholds
@@ -1209,6 +1235,24 @@ static int do_reduce(const void* send, void* recv, size_t count, int dtype, int 
              : (g->heap.mc_base && nvls_supports(dtype, op) && n >= g->nvls_min_ranks) ? B200MPI_ALGO_NVLS : B200MPI_ALGO_TWOSHOT;
   if ((rc = launch_reduce(algo, dtype, op, st.in, st.out, count, root, g->stream))) return rc;
   return finish(async, st);
+}
+
+// Scan: rank r's recv = send_0 op ... op send_r, in rank order.  Exscan (exclusive): the same up to
+// send_{r-1}; rank 0's recv is not written and may be NULL.  One algorithm, no host pipelining: host
+// slices and foreign device pointers are staged whole.
+static int do_scan(const void* send, void* recv, size_t count, int dtype, int op, int memkind, bool exclusive) {
+  const char* what = exclusive ? "exscan" : "scan";
+  size_t es;
+  int rc = check_coll(what, kReduces, dtype, op, 0, memkind, es);
+  if (rc) return rc;
+  const bool gets = !exclusive || g->ctrl.rank > 0; // this rank's recv is written
+  if (count && (!send || (gets && !recv))) return null_buffer(what);
+  const size_t bytes = count * es;
+  if (g->ctrl.n == 1) return gets ? local_copy(recv, send, bytes, memkind, false) : finish(false);
+  Staging st;
+  if ((rc = stage(st, memkind, send, bytes, recv, bytes, !gets ? kSendOnly : recv == send ? kRecvInSend : kApart))) return rc;
+  if ((rc = launch_scan(exclusive, dtype, op, st.in, st.out, count, g->stream))) return rc;
+  return finish(false, st);
 }
 
 // Alltoall: send and recv hold size()*count elements; block j of send goes to rank j's block rank().
@@ -2075,6 +2119,8 @@ int b200mpi_allgather(const void* send, void* recv, size_t count, int dtype, int
 int b200mpi_reduce_scatter(const void* send, void* recv, size_t count_per_rank, int dtype, int op, int memkind) { return do_reduce_scatter(send, recv, count_per_rank, dtype, op, memkind, false); }
 int b200mpi_reduce(const void* send, void* recv, size_t count, int dtype, int op, int root, int memkind) { return do_reduce(send, recv, count, dtype, op, root, memkind, false); }
 int b200mpi_alltoall(const void* send, void* recv, size_t count_per_rank, int dtype, int memkind) { return do_alltoall(send, recv, count_per_rank, dtype, memkind, false); }
+int b200mpi_scan(const void* send, void* recv, size_t count, int dtype, int op, int memkind) { return do_scan(send, recv, count, dtype, op, memkind, false); }
+int b200mpi_exscan(const void* send, void* recv, size_t count, int dtype, int op, int memkind) { return do_scan(send, recv, count, dtype, op, memkind, true); }
 int b200mpi_gather(const void* send, void* recv, size_t count_per_rank, int dtype, int root, int memkind) { return do_gather(send, recv, count_per_rank, dtype, root, memkind, false); }
 int b200mpi_scatter(const void* send, void* recv, size_t count_per_rank, int dtype, int root, int memkind) { return do_gather(send, recv, count_per_rank, dtype, root, memkind, true); }
 int b200mpi_gatherv(const void* send, void* recv, const size_t* counts, int dtype, int root, int memkind) { return do_gatherv(send, recv, counts, dtype, root, false, memkind); }

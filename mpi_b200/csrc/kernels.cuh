@@ -660,6 +660,103 @@ allreduce_twoshot_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t co
 }
 
 // ---------------------------------------------------------------------------------------------
+// Scan / Exscan: prefix reductions in rank order.  Rank r receives ((x_0 op x_1) op ...) op x_r
+// (Scan) or the same up to x_{r-1} (Exscan; rank 0 receives nothing).  Same ownership and traffic
+// as the two-shot Allreduce: the owner of a vector loads it from every rank's send (Exscan never
+// needs rank n-1's), forms the running prefix in registers and stores prefix r (r-1) into rank r's
+// recv, starting at the next rank.  In place is safe for the same reason as in two-shot.  Under
+// Exscan rank 0 announces its send offset as its recv, and nothing is ever stored to rank 0.
+// ---------------------------------------------------------------------------------------------
+// One element e, scalar, in rank order: the unaligned body and the tail past the last whole vector.
+// Rank r's input is loaded before rank r's recv is stored, so in place holds here too.
+template <typename T, typename Op, bool EXCLUSIVE>
+__device__ __forceinline__ void scan_element(const Comm& c, const uint64_t* s_a, const uint64_t* s_b, int n, size_t e) {
+  auto in = [&](int r) { return reinterpret_cast<const volatile T*>(c.base[r] + s_a[r])[e]; };
+  auto out = [&](int r, T v) { reinterpret_cast<volatile T*>(c.base[r] + s_b[r])[e] = v; };
+  T acc = in(0);
+  if (!EXCLUSIVE) out(0, acc);
+  for (int r = 1; r < n; ++r) {
+    if (EXCLUSIVE) {
+      const T x = r < n - 1 ? in(r) : T(0);
+      out(r, acc);
+      if (r < n - 1) acc = Op::template apply<T>(acc, x);
+    } else {
+      acc = Op::template apply<T>(acc, in(r));
+      out(r, acc);
+    }
+  }
+}
+
+template <typename T, typename Op, int NR, int UNROLL, bool EXCLUSIVE>
+__global__ void __launch_bounds__(kThreads, 1)
+scan_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t count, uint32_t shift) {
+  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
+  const bool call_ok = sync_start(c, send_off, recv_off, s_a, s_b);
+  if (!call_ok) { // ranks disagree about this call: touch nothing, leave through the end barrier
+    sync_end_failed(c);
+    return;
+  }
+  const int n = NR ? NR : c.n;
+  const int nin = EXCLUSIVE ? n - 1 : n; // ranks whose input any result needs
+  constexpr int R = NR ? NR : kMaxRanks;
+  constexpr int EPV = Pack<T>::N;
+  const size_t tid = threadIdx.x;
+  const size_t nthreads = (size_t)gridDim.x * blockDim.x;
+  if (all_aligned16(s_a, s_b, n)) {
+    const size_t nvec = count / EPV;
+    const Owner own(nvec, shift, n, c.rank);
+    __shared__ const char* src[kMaxRanks];
+    __shared__ char* dst[kMaxRanks];
+    if (tid < (size_t)R) {
+      const int r = (int)tid < n ? (int)tid : 0;
+      src[tid] = c.base[r] + s_a[r];
+      dst[tid] = c.base[r] + s_b[r];
+    }
+    __syncthreads();
+    const size_t step = nthreads * UNROLL;
+    for (size_t l0 = (size_t)blockIdx.x * blockDim.x * UNROLL + tid; l0 < own.slots; l0 += step) {
+      Pack<T> v[UNROLL][R];
+      size_t gi[UNROLL];
+#pragma unroll
+      for (int u = 0; u < UNROLL; ++u) {
+        const size_t l = l0 + (size_t)u * blockDim.x;
+        gi[u] = l < own.slots ? own.global(l) : nvec;
+        if (gi[u] < nvec) {
+#pragma unroll
+          for (int r = 0; r < R; ++r)
+            if (r < nin) v[u][r] = ld_pack<T>(src[r] + gi[u] * 16);
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < UNROLL; ++u) {
+        if (gi[u] < nvec) {
+#pragma unroll
+          for (int r = 1; r < R; ++r) // v[u][r] becomes prefix r
+            if (r < nin) v[u][r] = combine<T, Op>(v[u][r - 1], v[u][r]);
+          // rank r's result is prefix r (Scan) or prefix r-1 (Exscan); ranks after this one first
+#pragma unroll
+          for (int r = EXCLUSIVE ? 1 : 0; r < R; ++r)
+            if (r > c.rank && r < n) st_pack<T>(dst[r] + gi[u] * 16, v[u][EXCLUSIVE ? r - 1 : r]);
+#pragma unroll
+          for (int r = EXCLUSIVE ? 1 : 0; r < R; ++r)
+            if (r <= c.rank) st_pack<T>(dst[r] + gi[u] * 16, v[u][EXCLUSIVE ? r - 1 : r]);
+        }
+      }
+    }
+    // elements past the last whole vector: reduced and pushed by the last rank
+    if (c.rank == n - 1)
+      for (size_t e = nvec * EPV + (size_t)blockIdx.x * blockDim.x + tid; e < count; e += nthreads) scan_element<T, Op, EXCLUSIVE>(c, s_a, s_b, n, e);
+  } else {
+    // unaligned buffers: contiguous ownership by element, scalar accesses
+    const size_t per = (count + n - 1) / n;
+    const size_t lo = per * c.rank < count ? per * c.rank : count;
+    const size_t hi = lo + per < count ? lo + per : count;
+    for (size_t e = lo + (size_t)blockIdx.x * blockDim.x + tid; e < hi; e += nthreads) scan_element<T, Op, EXCLUSIVE>(c, s_a, s_b, n, e);
+  }
+  sync_end(c);
+}
+
+// ---------------------------------------------------------------------------------------------
 // Allreduce, two-shot with shared-memory staging (TMA bulk copies).  Same ownership, traffic and
 // rank-order arithmetic as allreduce_twoshot_kernel, but the SM's load/store units never touch
 // NVLink: one producer thread per CTA streams kChunk-byte tiles of slice j from all NR heaps into

@@ -329,6 +329,46 @@ def main():
         sbuf.free()
         rbuf.free()
 
+    prefix = [c for c in ("scan", "exscan") if c in colls]
+    if prefix:
+        # One algorithm, blocking calls: time = events around back-to-back calls, max over ranks.  Both
+        # move the bytes of a two-shot Allreduce of the same size: per GPU (n-1)/n*S read from peers and
+        # (n-1)/n*S pushed to them, so the bound is 2(n-1)/n*S at 450 GB/s per direction (H100 SXM data
+        # sheet), and a two-shot Allreduce of the same size is timed in the same run next to each.
+        if n < 2 or L.get_param("shared_device"):
+            emit({"coll": "scan", "ok": True, "note": "fewer than two NVLink-connected GPUs (ranks %s): Scan / Exscan bandwidth not measured"
+                  % ("share one GPU" if n > 1 else "= 1")})
+        else:
+            per_max = min(args.max_bytes, 512 << 20)
+            send = mpi.Alloc(per_max // 4, np.float32).copy_from_host(np.full(per_max // 4, rank + 1, dtype=np.float32))
+            recv = mpi.Alloc(per_max // 4, np.float32)
+            link = 450e9
+            lib.b200mpi_set_algo(L.COLL_ALLREDUCE, ALGOS["twoshot"])
+            for S in [s for s in sizes if s <= per_max]:
+                cnt = S // 4
+                it, wm = iters_for(S)
+                bound = 2 * (n - 1) / n * S / link
+                t_ar = timed(lambda: lib.b200mpi_allreduce_async(send.ptr, recv.ptr, cnt, L.F32, L.SUM), it, wm)
+                for coll in prefix:
+                    fn = lib.b200mpi_exscan if coll == "exscan" else lib.b200mpi_scan
+
+                    def blocking():
+                        if fn(send.ptr, recv.ptr, cnt, L.F32, L.SUM, L.DEVICE):
+                            raise RuntimeError(L.last_error())
+                    recv[:min(cnt, 64)].copy_from_host(np.full(min(cnt, 64), -1, dtype=np.float32))
+                    t = timed(blocking, it, wm)
+                    # x_r = r + 1: rank r holds (r+1)(r+2)/2 after Scan, r(r+1)/2 after Exscan (rank 0: untouched)
+                    k = rank if coll == "exscan" else rank + 1
+                    want = np.float32(k * (k + 1) // 2) if k else np.float32(-1)
+                    probe = recv[:min(cnt, 64)].to_host()
+                    ok = maxr(0.0 if bool(np.all(probe == want)) else 1.0) == 0.0
+                    emit({"coll": coll, "dtype": "f32", "algo": "owner", "bytes": S, "t_us": t * 1e6, "algbw_gbs": S / t / 1e9,
+                          "link_bytes": 2 * (n - 1) / n * S, "link_roofline_share": bound / t,
+                          "twoshot_allreduce_t_us": t_ar * 1e6, "vs_twoshot_allreduce": t_ar / t, "ok": ok})
+            lib.b200mpi_set_algo(L.COLL_ALLREDUCE, 0)
+            send.free()
+            recv.free()
+
     if "p2p" in colls and n > 1:
         # bounce (examples/bounce/bounce.go:85-138): even sends, odd returns; device-resident float64
         maxp = min(args.max_bytes, 256 << 20)

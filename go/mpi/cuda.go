@@ -471,6 +471,21 @@ func resized(what string, recv interface{}, n int) (interface{}, error) {
 	return nil, fmt.Errorf("mpi: %s needs a pointer to []float64, []float32, []int64, []byte or Raw, or a *DeviceSlice, got %T", what, recv)
 }
 
+// lenOf is the element count of a recv passed as a pointer to a slice or as a *DeviceSlice.
+func lenOf(recv interface{}) (int, bool) {
+	switch v := recv.(type) {
+	case *[]float64:
+		return len(*v), true
+	case *[]float32:
+		return len(*v), true
+	case *[]int64:
+		return len(*v), true
+	case *DeviceSlice:
+		return v.Len, true
+	}
+	return 0, false
+}
+
 // table checks counts against Size() and returns it as the C array.
 func (c *Cuda) table(what string, counts []int) ([]C.size_t, int, error) {
 	if len(counts) != c.Size() {
@@ -626,6 +641,47 @@ func (c *Cuda) Gatherv(send, recv interface{}, counts []int, root int) ([]int, e
 
 func (c *Cuda) Allgatherv(send, recv interface{}, counts []int) ([]int, error) {
 	return c.gatherv("Allgatherv", send, recv, counts, 0, true)
+}
+
+// ReduceScatterv: rank j's recv, resized to counts[j], receives op over every rank's block j in rank
+// order. A nil counts on every rank is learnt from len(recv) with one Allgather. In place: recv points
+// at this rank's block of send.
+func (c *Cuda) ReduceScatterv(send, recv interface{}, counts []int, op Op) ([]int, error) {
+	sp, sn, sdt, sk, err := lowerTyped("ReduceScatterv", send)
+	if err != nil {
+		return nil, err
+	}
+	if counts == nil {
+		rn, ok := lenOf(recv)
+		if !ok {
+			return nil, fmt.Errorf("mpi: ReduceScatterv learns counts from a pointer to []float64, []float32 or []int64, or a *DeviceSlice, got %T", recv)
+		}
+		if counts, err = c.lengths(rn); err != nil {
+			return nil, err
+		}
+	}
+	t, total, err := c.table("ReduceScatterv", counts)
+	if err != nil {
+		return nil, err
+	}
+	if total != sn {
+		return nil, errors.New("mpi: ReduceScatterv send must hold sum(counts) elements")
+	}
+	r, err := resized("ReduceScatterv", recv, counts[c.Rank()])
+	if err != nil {
+		return nil, err
+	}
+	rp, _, rdt, rk, err := lowerTyped("ReduceScatterv", r)
+	if err != nil {
+		return nil, err
+	}
+	if sdt != rdt || sk != rk {
+		return nil, errors.New("mpi: ReduceScatterv send and recv must have the same type and memory kind")
+	}
+	if rc := C.b200mpi_reduce_scatterv(sp, rp, &t[0], sdt, C.int(op), sk); rc != 0 {
+		return nil, lastError(rc, 0)
+	}
+	return counts, nil
 }
 
 // Scatterv: root always sends its table with one small Bcast, so the other ranks may pass nil.

@@ -28,6 +28,7 @@
 //	Gatherv, Scatterv, Allgatherv     the same with a different length on every rank
 //	Alltoallv                         Alltoall with a different length for every (source, destination) pair
 //	Scan, Exscan                      prefix reductions in rank order (inclusive, exclusive)
+//	ReduceScatterv                    ReduceScatter with a different block length for every rank
 //	Isend + Wait   the non-blocking Send design the reference sketches and comments out (mpi.go:132-152)
 //
 // They are served through the optional Collective interface, the upgrade the reference hints at
@@ -94,6 +95,11 @@ type Collective4 interface {
 type Collective5 interface {
 	Scan(send, recv interface{}, op Op) error
 	Exscan(send, recv interface{}, op Op) error
+}
+
+// Collective6 is the sixth optional upgrade: the reduce-scatter whose blocks follow a counts table.
+type Collective6 interface {
+	ReduceScatterv(send, recv interface{}, counts []int, op Op) ([]int, error)
 }
 
 // Raw marks a payload that is sent as bytes without any encoding.
@@ -353,4 +359,17 @@ func Exscan(send, recv interface{}, op Op) error {
 		return err
 	}
 	return c.Exscan(send, recv, op)
+}
+
+// ReduceScatterv reduces block j of every rank's send (counts[j] elements at offset
+// counts[0]+...+counts[j-1]; send holds sum(counts)) with op, in rank order, into rank j's recv,
+// which is resized to counts[j]. A nil counts on every rank is learnt from len(recv) with one
+// Allgather, and the table used is returned. In place: recv points at this rank's block of send,
+// the form an in-place Allgatherv with the same table completes into an Allreduce.
+func ReduceScatterv(send, recv interface{}, counts []int, op Op) ([]int, error) {
+	c, ok := current.(Collective6)
+	if !ok {
+		return nil, fmt.Errorf("mpi: registered implementation %T has no ReduceScatterv", current)
+	}
+	return c.ReduceScatterv(send, recv, counts, op)
 }

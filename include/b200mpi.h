@@ -31,8 +31,8 @@ extern "C" {
 #endif
 
 #define B200MPI_VERSION 200 /* 0.2.0: + isend/wait, reduce_scatter, reduce, alltoall, probes, get_param;
-                               then gather, scatter, gatherv, scatterv, allgatherv, alltoallv, scan, exscan
-                               (all additive) */
+                               then gather, scatter, gatherv, scatterv, allgatherv, alltoallv, scan, exscan,
+                               reduce_scatterv (all additive) */
 #define B200MPI_MAX_RANKS 8 /* "the 8 GPUs of one box" */
 
 typedef enum {
@@ -177,6 +177,13 @@ int b200mpi_scan(const void* send, void* recv, size_t count, int dtype, int op, 
  * (it may be NULL there; in place, rank 0 keeps its input).  For both, buffers outside the
  * b200mpi_alloc heap are staged whole through it (B200MPI_ERR_NOMEM if too big). */
 int b200mpi_exscan(const void* send, void* recv, size_t count, int dtype, int op, int memkind);
+/* send holds sum(counts) elements; rank j receives op over r of rank r's block j, combined left to
+ * right in rank order.  Block j starts at displacement counts[0] + ... + counts[j-1] of every send;
+ * recv holds counts[rank()] elements and may be NULL where that is 0.  counts is the same table on
+ * every rank (a rank whose table differs gets B200MPI_ERR_PEER, as do all others).  In place: recv ==
+ * send + displ[rank()] (the form in-place Allgatherv completes).  Buffers outside the b200mpi_alloc
+ * heap are staged whole through it (B200MPI_ERR_NOMEM if too big). */
+int b200mpi_reduce_scatterv(const void* send, void* recv, const size_t* counts, int dtype, int op, int memkind);
 int b200mpi_barrier(void);
 
 /* Enqueue-only forms on the library stream (DEVICE memkind only). */

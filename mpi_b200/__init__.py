@@ -3,13 +3,13 @@
 `import mpi_b200 as mpi` gives the reference's package surface (mpi.go) over libb200mpi.so:
 Init, Finalize, Rank, Size, Send, Receive (+ Recv, Bcast, Allreduce, Allgather, Barrier,
 ReduceScatter, Reduce, Alltoall, Gather, Scatter, Gatherv, Scatterv, Allgatherv, Alltoallv,
-Scan, Exscan, Isend/Wait).
+Scan, Exscan, ReduceScatterv, Isend/Wait).
 The shared library (mpi_b200/lib/libb200mpi.so, built by mpi_b200/csrc/Makefile) is loaded on
 first use; nothing here computes or moves payload bytes in Python.
 """
 from ._lib import LIB_PATH, load  # noqa: F401
 from .api import (  # noqa: F401
     MAX, MIN, SUM, Alloc, Allgather, Allgatherv, Allreduce, Alltoall, Alltoallv, Barrier, Bcast, Cuda, DeviceSlice, Exscan,
-    Finalize, Gather, Gatherv, Init, Interface, Isend, MpiError, Rank, Raw, Receive, Recv, Reduce, ReduceScatter, Register,
-    Scan, Scatter, Scatterv, Send, Size, TagExists, Wait)
+    Finalize, Gather, Gatherv, Init, Interface, Isend, MpiError, Rank, Raw, Receive, Recv, Reduce, ReduceScatter,
+    ReduceScatterv, Register, Scan, Scatter, Scatterv, Send, Size, TagExists, Wait)
 from . import flags  # noqa: F401

@@ -10,6 +10,7 @@ Same names, same argument meaning, same blocking behaviour:
     Gather(send, recv, root)  Scatter(send, recv, root)                                       (new)
     Gatherv(send, recv, root, counts)  Scatterv(send, recv, counts, root)  Allgatherv(send, recv, counts)
     Alltoallv(send, send_counts, recv, recv_counts)                                          (new)
+    ReduceScatterv(send, recv, counts, op)                                                   (new)
     Isend(data, destination, tag) + Wait(destination, tag)     (the Send/Wait design commented out
                                                                 in the reference, mpi.go:132-152)
 
@@ -477,6 +478,25 @@ class Cuda(Interface):
         _check(L.load().b200mpi_alltoallv(sp, stable, rp, rtable, sdt, sk))
         return recv, recv_counts
 
+    def ReduceScatterv(self, send, recv=None, counts=None, op=SUM):
+        """Rank j's recv receives op over every rank's block j, combined in rank order; block j is
+        counts[j] elements at displacement counts[0]+...+counts[j-1] of send (sum(counts) elements).
+        counts is the same table on every rank; omitted on every rank, it is learnt from len(recv)
+        with one Allgather.  A host recv is created or resized as in Gatherv.  In place: recv is
+        this rank's block of send.  Returns (recv, counts)."""
+        rank, n = self._world()
+        sp, sc, sdt, sk, keep, _ = _describe(send)
+        if counts is None:
+            if recv is None:
+                raise ValueError("mpi: ReduceScatterv needs counts or a recv to learn them from")
+            counts = self._lengths(_describe(recv)[1])
+        counts, table = self._table(counts, n)
+        if sum(counts) != sc:
+            raise ValueError("mpi: ReduceScatterv send must hold sum(counts) elements")
+        recv, rp = self._recv_for(recv, counts[rank], sdt, sk, "ReduceScatterv")
+        _check(L.load().b200mpi_reduce_scatterv(sp, rp, table, sdt, int(op), sk))
+        return recv, counts
+
 
 # ---- package-level facade: mpi.go:56-159 -------------------------------------------------------
 _mpier = Cuda()
@@ -590,6 +610,10 @@ def Allgatherv(send, recv=None, counts=None):
 
 def Alltoallv(send, send_counts, recv=None, recv_counts=None):
     return _collective("Alltoallv")(send, send_counts, recv, recv_counts)
+
+
+def ReduceScatterv(send, recv=None, counts=None, op=SUM):
+    return _collective("ReduceScatterv")(send, recv, counts, op)
 
 
 def Isend(data, destination, tag):

@@ -14,7 +14,7 @@
 //   mpi.Register(impl)                         void mpi::Register(Interface*)  (second call throws = panics, mpi.go:61-67)
 //   flag.Parse() + mpi.Flag*                   mpi::ParseFlags(argc, argv) + mpi::Flag*
 //   new: Recv, Bcast, Allreduce, Allgather, Barrier, ReduceScatter, Reduce, Alltoall, Isend/Wait,
-//        Gather, Scatter, Gatherv, Scatterv, Allgatherv, Alltoallv, Scan, Exscan;
+//        Gather, Scatter, Gatherv, Scatterv, Allgatherv, Alltoallv, Scan, Exscan, ReduceScatterv;
 //        mpi::DeviceSlice<T> for heap-resident buffers
 // `data` may be std::vector<double|float|int64_t|uint8_t>, std::string (sent as bytes, the
 // "anything else is gob-encoded" path), or DeviceSlice<T>.
@@ -186,6 +186,8 @@ struct Interface {
   virtual Error Allgatherv(Buffer, Buffer, const size_t*) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Allgatherv"; return e; }
   // send_counts / recv_counts[Size()]: this rank's row and column of the exchange (they differ from rank to rank)
   virtual Error Alltoallv(Buffer, const size_t*, Buffer, const size_t*) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Alltoallv"; return e; }
+  // counts[Size()] is the same table on every rank: rank j receives the reduction of block j
+  virtual Error ReduceScatterv(Buffer, Buffer, const size_t*, Op) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no ReduceScatterv"; return e; }
   // the Send/Wait pair the reference sketches and comments out (mpi.go:132-152)
   virtual Error Isend(Buffer, int, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Isend"; return e; }
   virtual Error Wait(int, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Wait"; return e; }
@@ -228,6 +230,7 @@ struct Cuda : Interface {
   Error Scatterv(Buffer s, Buffer r, const size_t* counts, int root) override { return make_error(b200mpi_scatterv(s.ptr, r.ptr, counts, r.dtype, root, r.memkind)); }
   Error Allgatherv(Buffer s, Buffer r, const size_t* counts) override { return make_error(b200mpi_allgatherv(s.ptr, r.ptr, counts, s.dtype, s.memkind)); }
   Error Alltoallv(Buffer s, const size_t* sc, Buffer r, const size_t* rc) override { return make_error(b200mpi_alltoallv(s.ptr, sc, r.ptr, rc, s.dtype, s.memkind)); }
+  Error ReduceScatterv(Buffer s, Buffer r, const size_t* counts, Op op) override { return make_error(b200mpi_reduce_scatterv(s.ptr, r.ptr, counts, s.dtype, op, s.memkind)); }
   Error Isend(Buffer d, int destination, int tag) override { return make_error(b200mpi_isend(d.ptr, d.count, d.dtype, destination, tag, d.memkind)); }
   Error Wait(int destination, int tag) override { return make_error(b200mpi_wait(destination, tag)); }
 };
@@ -399,6 +402,19 @@ template <typename T> inline Error Alltoallv(const std::vector<T>& send, const s
   if (n > 0 && recv_counts->size() != n) return arg_error("mpi: Alltoallv recv_counts must hold Size() entries");
   recv->resize(sum_of(*recv_counts));
   return mpier()->Alltoallv(lower(send), send_counts.data(), lower(*recv), recv_counts->data());
+}
+
+// ReduceScatterv: send holds sum(counts) elements; rank j receives op over every rank's block j, in
+// rank order.  *recv is resized to counts[Rank()], as Allgatherv resizes.
+template <typename T> inline Error ReduceScatterv(const std::vector<T>& send, std::vector<T>* recv, const std::vector<size_t>& counts, Op op = SUM) {
+  const size_t n = (size_t)(Size() > 0 ? Size() : 0);
+  if (n > 0 && counts.size() != n) return arg_error("mpi: ReduceScatterv counts must hold Size() entries");
+  if (n > 0 && sum_of(counts) != send.size()) return arg_error("mpi: ReduceScatterv send must hold sum(counts) elements");
+  if (n > 0) recv->resize(counts[(size_t)Rank()]);
+  return mpier()->ReduceScatterv(lower(send), lower(*recv), counts.data(), op);
+}
+template <typename T> inline Error ReduceScatterv(const DeviceSlice<T>& send, DeviceSlice<T>* recv, const std::vector<size_t>& counts, Op op = SUM) {
+  return mpier()->ReduceScatterv(lower(send), lower(*recv), counts.data(), op);
 }
 
 template <typename D> inline Error Isend(const D& data, int destination, int tag) { return mpier()->Isend(lower(data), destination, tag); }

@@ -319,7 +319,8 @@ static int check_status() {
 // call.  coll: 0 allreduce, 1 bcast, 2 allgather, 3 barrier, 4 reduce_scatter, 5 reduce, 6 alltoall,
 // 7 gather(v), 8 scatter(v), 9 allgatherv (these three carry a hash of the counts table in `total`),
 // 10 alltoallv (whose ranks hold different tables: each adds its table digest to the signature it
-// announces, see sync_start_pairs in kernels.cuh), 11 scan, 12 exscan.
+// announces, see sync_start_pairs in kernels.cuh), 11 scan, 12 exscan, 13 reduce_scatterv (which
+// carries the table hash in `total`, as 7-9 do).
 // `total` is the element count of the whole user call when the launch is one chunk of a pipelined
 // host-slice call (ranks that disagree about the total then disagree from the first chunk on).
 static uint64_t make_sig(int coll, int dtype, int extra, int algo, size_t count, size_t total = 0) {
@@ -1295,10 +1296,10 @@ static int make_vtable(const char* what, const size_t* counts, size_t es, VTable
 }
 
 // The grid of a table-driven launch follows the largest block, so every rank launches the same one.
-static int vtable_grid(const VTable& vt) {
+static int vtable_grid(const VTable& vt, int unroll = 4) {
   size_t largest = 0;
   for (int r = 0; r < g->ctrl.n; ++r) largest = std::max<size_t>(largest, vt.off[r + 1] - vt.off[r]);
-  return grid_for(largest / 16 + 1, 4);
+  return grid_for(largest / 16 + 1, unroll);
 }
 
 // OR of the displacements off[0..n]: with this rank's offsets they pick its access unit (with_unit).
@@ -1357,6 +1358,44 @@ static int do_scatterv(const void* send, void* recv, const size_t* counts, int d
     return launch_coll(scatterv_pull_kernel<decltype(u), 4>, "scatterv_pull_kernel", sig, blocks, kThreads, 0, g->stream, st.in, st.out, vt, root);
   });
   return rc ? rc : finish(false, st);
+}
+
+// ReduceScatterv: one algorithm, the grid of the largest block.  UNROLL per element size is the
+// largest power of two for which ptxas reports no spill in any instance.  The signature carries the
+// total count and the table hash, so a rank with another table, op or dtype, or one calling
+// ReduceScatter (code 4), ends the call as B200MPI_ERR_PEER on every rank.
+static int launch_reduce_scatterv(int dtype, int op, uint64_t so, uint64_t ro, const VTable& vt, size_t es, uint64_t hash, cudaStream_t s) {
+  const uint64_t sig = make_sig(13, dtype, op, 0, vt.off[g->ctrl.n] / es, hash);
+  return with_reduction(
+      dtype, op,
+      [&](auto t, auto o) {
+        using T = decltype(t);
+        using Op = decltype(o);
+        constexpr int U = sizeof(T) == 4 ? 8 : 4; // f64 min/max spilled at 8, every type at 16
+        return launch_coll(reduce_scatterv_kernel<T, Op, U>, "reduce_scatterv_kernel", sig, vtable_grid(vt, U), kThreads, 0, s, so, ro, vt);
+      },
+      [] { return fail(B200MPI_ERR_UNSUPPORTED, "reduce_scatterv: unsupported dtype/op (need f32, f64 or i64 with sum/max/min)"); });
+}
+
+// ReduceScatterv: send holds sum(counts) elements; rank j's recv (counts[j] elements, NULL allowed
+// when that is 0) receives op over r of block j of rank r's send.  In place: recv == send + the
+// displacement of this rank's block.  Host slices and foreign device pointers are staged whole.
+static int do_reduce_scatterv(const void* send, void* recv, const size_t* counts, int dtype, int op, int memkind) {
+  size_t es;
+  int rc = check_coll("reduce_scatterv", kReduces, dtype, op, 0, memkind, es);
+  if (rc) return rc;
+  const int n = g->ctrl.n, me = g->ctrl.rank;
+  VTable vt;
+  uint64_t hash;
+  if ((rc = make_vtable("reduce_scatterv", counts, es, vt, hash))) return rc;
+  const size_t mine = vt.off[me + 1] - vt.off[me], total = vt.off[n];
+  if ((total && !send) || (mine && !recv)) return null_buffer("reduce_scatterv");
+  if (n == 1) return local_copy(recv, send, mine, memkind, false); // counts[0] covers the whole send
+  const bool inplace = recv && (const char*)recv == (const char*)send + vt.off[me];
+  Staging st; // a NULL recv (counts[rank] == 0) announces the send offset and is never written
+  if ((rc = stage(st, memkind, send, total, recv, mine, !recv ? kSendOnly : inplace ? kRecvInSend : kApart, vt.off[me]))) return rc;
+  if ((rc = launch_reduce_scatterv(dtype, op, st.in, st.out, vt, es, hash, g->stream))) return rc;
+  return finish(false, st);
 }
 
 // The fixed-count forms: the uniform table.
@@ -2126,6 +2165,9 @@ int b200mpi_scatter(const void* send, void* recv, size_t count_per_rank, int dty
 int b200mpi_gatherv(const void* send, void* recv, const size_t* counts, int dtype, int root, int memkind) { return do_gatherv(send, recv, counts, dtype, root, false, memkind); }
 int b200mpi_scatterv(const void* send, void* recv, const size_t* counts, int dtype, int root, int memkind) { return do_scatterv(send, recv, counts, dtype, root, memkind); }
 int b200mpi_allgatherv(const void* send, void* recv, const size_t* counts, int dtype, int memkind) { return do_gatherv(send, recv, counts, dtype, 0, true, memkind); }
+int b200mpi_reduce_scatterv(const void* send, void* recv, const size_t* counts, int dtype, int op, int memkind) {
+  return do_reduce_scatterv(send, recv, counts, dtype, op, memkind);
+}
 int b200mpi_alltoallv(const void* send, const size_t* send_counts, void* recv, const size_t* recv_counts, int dtype, int memkind) {
   return do_alltoallv(send, send_counts, recv, recv_counts, dtype, memkind);
 }

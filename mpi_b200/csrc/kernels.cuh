@@ -1687,6 +1687,103 @@ scatterv_pull_kernel(Comm c, uint64_t send_off, uint64_t recv_off, VTable vt, in
 }
 
 // ---------------------------------------------------------------------------------------------
+// ReduceScatterv: rank j receives op over r of block j of rank r's send, combined in rank order,
+// where block j is [off[j], off[j+1]) of every send (VTable).  Only rank j reads block j, and each
+// element of it is loaded from every rank, reduced and stored by one thread, so recv may be block j
+// of rank j's own send (in place) with no mid barrier: the other ranks read only blocks k != j.
+// A displacement from a table is rarely a multiple of 16 bytes, so the block is split at the first
+// 16-byte boundary of its source addresses (split16): the head and tail elements go one T at a time,
+// the whole vectors 16 bytes at a time, as long as the n sources agree mod 16 (heap and staged sends
+// are 512-byte aligned and share the displacement, so they usually do).  The vectors are stored 16
+// bytes wide when recv has the sources' residue and one T at a time otherwise.  Sources that disagree
+// mod 16 leave the whole block to scalar element ownership.
+// ---------------------------------------------------------------------------------------------
+// `count` elements of `es` bytes from address `addr`: `head` elements up to the first 16-byte
+// boundary, `nvec` whole 16-byte vectors from there, `tail` elements after them.  An address that is
+// not a multiple of `es` never reaches a boundary on an element edge: everything is head.
+struct Split16 {
+  size_t head, nvec, tail;
+};
+__host__ __device__ __forceinline__ Split16 split16(uint64_t addr, size_t count, size_t es) {
+  if (addr % es) return {count, 0, 0};
+  const size_t head = ((16 - (addr & 15)) & 15) / es;
+  if (head >= count) return {count, 0, 0};
+  const size_t epv = 16 / es;
+  const size_t nvec = (count - head) / epv;
+  return {head, nvec, count - head - nvec * epv};
+}
+
+// Element e of this rank's block, reduced over the n sources in rank order.
+template <typename T, typename Op>
+__device__ __forceinline__ T rsv_element(const char* const* src, int n, size_t e) {
+  T acc = reinterpret_cast<const volatile T*>(src[0])[e];
+  for (int r = 1; r < n; ++r) acc = Op::template apply<T>(acc, reinterpret_cast<const volatile T*>(src[r])[e]);
+  return acc;
+}
+
+template <typename T, typename Op, int UNROLL>
+__global__ void __launch_bounds__(kThreads, 1)
+reduce_scatterv_kernel(Comm c, uint64_t send_off, uint64_t recv_off, VTable vt) {
+  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
+  __shared__ const char* src[kMaxRanks];
+  const bool call_ok = sync_start(c, send_off, recv_off, s_a, s_b);
+  if (!call_ok) {
+    sync_end_failed(c);
+    return;
+  }
+  const int n = c.n;
+  constexpr int EPV = Pack<T>::N;
+  uint64_t lo, hi;
+  vtable_range(vt, c.rank, lo, hi);
+  if (threadIdx.x < (unsigned)n) src[threadIdx.x] = c.base[threadIdx.x] + s_a[threadIdx.x] + lo;
+  __syncthreads();
+  const size_t count = (hi - lo) / sizeof(T);
+  T* const out = reinterpret_cast<T*>(c.base[c.rank] + recv_off);
+  const uint64_t res = (send_off + lo) & 15;
+  bool agree = true;
+  for (int r = 0; r < n; ++r) agree = agree && ((s_a[r] + lo) & 15) == res;
+  const Split16 sp = agree ? split16(send_off + lo, count, sizeof(T)) : Split16{count, 0, 0};
+  const size_t tid = threadIdx.x;
+  const size_t gtid = (size_t)blockIdx.x * blockDim.x + tid, gstride = (size_t)gridDim.x * blockDim.x;
+  for (size_t e = gtid; e < sp.head; e += gstride) out[e] = rsv_element<T, Op>(src, n, e);
+  const size_t v0 = sp.head * sizeof(T); // byte offset of the first whole vector in every source
+  const bool wide_out = (recv_off & 15) == res;
+  const size_t step = gstride * UNROLL;
+  for (size_t i0 = (size_t)blockIdx.x * blockDim.x * UNROLL + tid; i0 < sp.nvec; i0 += step) {
+    Pack<T> acc[UNROLL];
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u) {
+      const size_t i = i0 + (size_t)u * blockDim.x;
+      if (i < sp.nvec) acc[u] = ld_pack<T>(src[0] + v0 + i * 16);
+    }
+    for (int r = 1; r < n; ++r) { // UNROLL vectors of rank r in flight, combined in rank order
+      Pack<T> v[UNROLL];
+#pragma unroll
+      for (int u = 0; u < UNROLL; ++u) {
+        const size_t i = i0 + (size_t)u * blockDim.x;
+        if (i < sp.nvec) v[u] = ld_pack<T>(src[r] + v0 + i * 16);
+      }
+#pragma unroll
+      for (int u = 0; u < UNROLL; ++u)
+        if (i0 + (size_t)u * blockDim.x < sp.nvec) acc[u] = combine<T, Op>(acc[u], v[u]);
+    }
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u) {
+      const size_t i = i0 + (size_t)u * blockDim.x;
+      if (i >= sp.nvec) continue;
+      if (wide_out) {
+        st_pack<T>(reinterpret_cast<char*>(out) + v0 + i * 16, acc[u]);
+      } else {
+#pragma unroll
+        for (int k = 0; k < EPV; ++k) out[sp.head + i * EPV + k] = acc[u].v[k];
+      }
+    }
+  }
+  for (size_t e = sp.head + sp.nvec * EPV + gtid; e < count; e += gstride) out[e] = rsv_element<T, Op>(src, n, e);
+  sync_end(c);
+}
+
+// ---------------------------------------------------------------------------------------------
 // Alltoallv: rank i holds its send row S_i[0..n) and its recv column R_i[0..n) of an n x n matrix of
 // block sizes; the call is consistent when R_j[i] == S_i[j] for every pair.  The tables differ from
 // rank to rank, so they cannot be hashed into one shared signature.  Instead rank i announces

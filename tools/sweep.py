@@ -369,6 +369,52 @@ def main():
             send.free()
             recv.free()
 
+    if "reduce_scatterv" in colls:
+        # One algorithm, blocking calls: time = events around back-to-back calls, max over ranks.  S =
+        # bytes of every rank's send.  Three tables: uniform (timed next to the P2P ReduceScatter of the
+        # same size), a balanced split of an indivisible count, and a skewed one (rank 0 holds half).
+        # Rank j reads its block c_j from n-1 peers and n-1 peers read theirs from it, so the per-GPU
+        # bound is the larger of ingress (n-1)*c_j and egress total - c_j, the busiest GPU over 450 GB/s
+        # per direction (H100 SXM data sheet).  x_r = r + 1, so every result element is n(n+1)/2.
+        if n < 2 or L.get_param("shared_device"):
+            emit({"coll": "reduce_scatterv", "ok": True, "note": "fewer than two NVLink-connected GPUs (ranks %s): ReduceScatterv bandwidth not measured"
+                  % ("share one GPU" if n > 1 else "= 1")})
+        else:
+            per_max = min(args.max_bytes, 512 << 20)
+            send = mpi.Alloc(per_max // 4 + n, np.float32).copy_from_host(np.full(per_max // 4 + n, rank + 1, dtype=np.float32))
+            recv = mpi.Alloc(per_max // 4 + n, np.float32)
+            link = 450e9
+            want = np.float32(n * (n + 1) // 2)
+            lib.b200mpi_set_algo(L.COLL_REDUCE_SCATTER, ALGOS["twoshot"])
+            for S in [s for s in sizes if 4 * n <= s <= per_max]:
+                cnt = S // 4 // n
+                odd = cnt * n + 1  # not a multiple of n
+                tables = {"uniform": [cnt] * n,
+                          "balanced": [odd // n + (1 if r < odd % n else 0) for r in range(n)],
+                          "skewed": [cnt * n // 2] + [(cnt * n - cnt * n // 2) // (n - 1)] * (n - 1)}
+                it, wm = iters_for(S)
+                t_rs = timed(lambda: lib.b200mpi_reduce_scatter_async(send.ptr, recv.ptr, cnt, L.F32, L.SUM), it, wm)
+                for shape, counts in tables.items():
+                    total = sum(counts)
+                    tab = (ctypes.c_size_t * n)(*counts)
+
+                    def blocking():
+                        if lib.b200mpi_reduce_scatterv(send.ptr, recv.ptr, tab, L.F32, L.SUM, L.DEVICE):
+                            raise RuntimeError(L.last_error())
+                    k = min(counts[rank], 64)
+                    recv[:k].copy_from_host(np.full(k, -1, dtype=np.float32))
+                    t = timed(blocking, it, wm)
+                    ok = maxr(0.0 if bool(np.all(recv[:k].to_host() == want)) else 1.0) == 0.0
+                    link_bytes = 4 * max(max((n - 1) * c, total - c) for c in counts)
+                    row = {"coll": "reduce_scatterv", "dtype": "f32", "algo": shape, "counts": counts, "bytes": total * 4, "t_us": t * 1e6,
+                           "algbw_gbs": total * 4 / t / 1e9, "link_bytes": link_bytes, "link_roofline_share": link_bytes / link / t, "ok": ok}
+                    if shape == "uniform":
+                        row.update({"reduce_scatter_t_us": t_rs * 1e6, "vs_reduce_scatter": t_rs / t})
+                    emit(row)
+            lib.b200mpi_set_algo(L.COLL_REDUCE_SCATTER, 0)
+            send.free()
+            recv.free()
+
     if "p2p" in colls and n > 1:
         # bounce (examples/bounce/bounce.go:85-138): even sends, odd returns; device-resident float64
         maxp = min(args.max_bytes, 256 << 20)

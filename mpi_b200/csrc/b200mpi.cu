@@ -391,6 +391,20 @@ static uint32_t own_shift(size_t nvec, int n, uint32_t min_shift) {
   return std::max(sh, min_shift);
 }
 
+template <int V> using ic = std::integral_constant<int, V>;
+
+// The template arguments (NR, UNROLL) of the owner-computes kernels, the two-shot Allreduce at its
+// default unroll and Scan, for a world of n ranks: f(NR, UNROLL) as integral constants.  NR = 0 is
+// the instance for any n.  UNROLL is the largest per (n, element size) for which ptxas reports no
+// spill: 8-byte min/max spilled at 8 vectors per thread.
+template <typename T, typename F>
+static int with_owner_tiling(int n, F&& f) {
+  if (n == 2) return f(ic<2>{}, ic<sizeof(T) == 4 ? 8 : 4>{});
+  if (n == 4) return f(ic<4>{}, ic<4>{});
+  if (n == 8) return f(ic<8>{}, ic<2>{});
+  return f(ic<0>{}, ic<1>{});
+}
+
 // only_dst: -1 allreduce, else the root of a Reduce (twoshot / nvls only)
 template <typename T, typename Op>
 static int launch_allreduce_body_t(int algo, uint64_t sig, uint64_t so, uint64_t ro, size_t count, int only_dst, cudaStream_t s) {
@@ -401,20 +415,14 @@ static int launch_allreduce_body_t(int algo, uint64_t sig, uint64_t so, uint64_t
   const uint32_t sh = own_shift(nvec, n, algo == B200MPI_ALGO_TWOSHOT_SMEM ? 8 : 0);
   switch (algo) {
     case B200MPI_ALGO_TWOSHOT: {
-#define B200_TWOSHOT(NRV, UV) \
-  return launch_coll(allreduce_twoshot_kernel<T, Op, NRV, UV>, "allreduce_twoshot_kernel", sig, grid_for(per, UV), kThreads, 0, s, so, ro, count, sh, only_dst);
-      if (g->twoshot_unroll) {
-        if (n == 2) B200_TWOSHOT(2, (sizeof(T) == 4 ? 8 : 4)) // 8-byte min/max spilled at 8 vectors per thread
-        else if (n == 4) B200_TWOSHOT(4, 4)
-        else if (n == 8) B200_TWOSHOT(8, 2)
-        else B200_TWOSHOT(0, 1)
-      } else {
-        if (n == 2) B200_TWOSHOT(2, 4)
-        else if (n == 4) B200_TWOSHOT(4, 2)
-        else if (n == 8) B200_TWOSHOT(8, 1)
-        else B200_TWOSHOT(0, 1)
-      }
-#undef B200_TWOSHOT
+      auto go = [&](auto nr, auto unroll) {
+        return launch_coll(allreduce_twoshot_kernel<T, Op, nr, unroll>, "allreduce_twoshot_kernel", sig, grid_for(per, unroll), kThreads, 0, s, so, ro, count, sh, only_dst);
+      };
+      if (g->twoshot_unroll) return with_owner_tiling<T>(n, go);
+      if (n == 2) return go(ic<2>{}, ic<4>{});
+      if (n == 4) return go(ic<4>{}, ic<2>{});
+      if (n == 8) return go(ic<8>{}, ic<1>{});
+      return go(ic<0>{}, ic<1>{});
     }
     case B200MPI_ALGO_RING:
       return launch_coll(allreduce_ring_kernel<T, Op>, "allreduce_ring_kernel", sig, grid_for(per, 4), kThreads, 0, s, so, ro, count);
@@ -610,8 +618,7 @@ static int launch_reduce_scatter(int algo, int dtype, int op, uint64_t so, uint6
       });
 }
 
-// Scan / Exscan: one algorithm, the two-shot ownership and grid.  UNROLL per (n, element size) is
-// the largest for which ptxas reports no spill in any instance.
+// Scan / Exscan: one algorithm, the two-shot ownership, grid and (NR, UNROLL).
 static int launch_scan(bool exclusive, int dtype, int op, uint64_t so, uint64_t ro, size_t count, cudaStream_t s) {
   const uint64_t sig = make_sig(exclusive ? 12 : 11, dtype, op, 0, count);
   return with_reduction(
@@ -625,13 +632,9 @@ static int launch_scan(bool exclusive, int dtype, int op, uint64_t so, uint64_t 
         const size_t per = (nvec + n - 1) / n;
         const uint32_t sh = own_shift(nvec, n, 0);
         auto go = [&](auto kernel, int unroll) { return launch_coll(kernel, "scan_kernel", sig, grid_for(per, unroll), kThreads, 0, s, so, ro, count, sh); };
-#define B200_SCAN(NRV, UV) \
-  return exclusive ? go(scan_kernel<T, Op, NRV, UV, true>, UV) : go(scan_kernel<T, Op, NRV, UV, false>, UV);
-        if (n == 2) B200_SCAN(2, (sizeof(T) == 4 ? 8 : 4))
-        else if (n == 4) B200_SCAN(4, 4)
-        else if (n == 8) B200_SCAN(8, 2)
-        else B200_SCAN(0, 1)
-#undef B200_SCAN
+        return with_owner_tiling<T>(n, [&](auto nr, auto unroll) {
+          return exclusive ? go(scan_kernel<T, Op, nr, unroll, true>, unroll) : go(scan_kernel<T, Op, nr, unroll, false>, unroll);
+        });
       },
       [&] { return fail(B200MPI_ERR_UNSUPPORTED, "scan: unsupported dtype/op (need f32, f64 or i64 with sum/max/min)"); });
 }

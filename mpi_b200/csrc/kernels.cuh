@@ -22,6 +22,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <type_traits>
 
 namespace b200 {
 
@@ -126,9 +127,20 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
+// 16-byte cells that carry their own flag words (start barrier slots, LL lanes)
+__device__ __forceinline__ void st_cell16(uint4* p, uint4 v) {
+  asm volatile("st.volatile.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+__device__ __forceinline__ uint4 ld_cell16(const uint4* p) {
+  uint4 v;
+  asm volatile("ld.volatile.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
+  return v;
+}
 
 // Spin until *p >= want (wrap-safe).  On watchdog expiry raises the host-visible status word
-// and gives up so the kernel can drain; the host then reports B200MPI_ERR_TIMEOUT.
+// and gives up so the kernel can drain; the host then reports B200MPI_ERR_TIMEOUT.  The poll is
+// written out here, in wait_cells and in allreduce_ll_kernel: shared through one helper it
+// compiled to different SASS in alltoallv_push_kernel and allreduce_ll_kernel.
 __device__ __forceinline__ bool wait_flag(const uint32_t* p, uint32_t want, const Comm& c) {
   unsigned long long t0 = 0;
   uint32_t it = 0;
@@ -150,25 +162,6 @@ __device__ __forceinline__ Slot* slot_of(const Comm& c, int owner, int block, in
   return reinterpret_cast<Slot*>(c.base[owner]) + (size_t)block * kMaxRanks + src;
 }
 
-// Per-CTA barrier #1: announce {a,b,sig} to every rank, wait for everyone's, publish the offsets
-// in smem.  Returns false when the body must not run:
-//   * a peer's signature differs from ours (status 2 -> B200MPI_ERR_PEER): ranks called different
-//     collectives / counts / types / grids, or
-//   * a peer did not show up within the watchdog time (status 1 -> B200MPI_ERR_TIMEOUT).
-// sync_end still runs, so nobody hangs, and no buffer is touched.
-// The signature covers the grid size.  CTAs other than 0 first look at what every peer's CTA 0
-// announced (slot row 0 of this rank's heap): if the peers launched a different grid, a CTA
-// without a partner learns it there instead of waiting for a flag that never comes.  (While the
-// grids match the row cannot be overwritten early: a peer's next kernel starts only after its
-// current one has finished, which needs this CTA to have passed sync_end.)
-__device__ __forceinline__ void st_cell16(uint4* p, uint4 v) {
-  asm volatile("st.volatile.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-__device__ __forceinline__ uint4 ld_cell16(const uint4* p) {
-  uint4 v;
-  asm volatile("ld.volatile.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
-  return v;
-}
 // Spin until the three cells of `s` carry `epoch`; values out through a/b/sig.  false on watchdog expiry.
 __device__ __forceinline__ bool wait_cells(const Slot* s, uint32_t epoch, const Comm& c, uint64_t& a, uint64_t& b, uint64_t& sig) {
   unsigned long long t0 = 0;
@@ -204,6 +197,32 @@ __device__ __forceinline__ int* start_verdict() {
   return &verdict;
 }
 
+// The last step of both start barriers, once every thread sees the final verdict: true when the
+// body may run; otherwise thread 0 raises status 2 (B200MPI_ERR_PEER) unless the watchdog has
+// already raised status 1.
+__device__ __forceinline__ bool start_agreed(const Comm& c) {
+  const int v = *start_verdict();
+  if (v) {
+    if (threadIdx.x == 0 && v != 3) {
+      *(volatile uint32_t*)c.status = 2u;
+      __threadfence_system();
+    }
+    return false;
+  }
+  return true;
+}
+
+// Per-CTA barrier #1: announce {a,b,sig} to every rank, wait for everyone's, publish the offsets
+// in smem.  Returns false when the body must not run:
+//   * a peer's signature differs from ours (status 2 -> B200MPI_ERR_PEER): ranks called different
+//     collectives / counts / types / grids, or
+//   * a peer did not show up within the watchdog time (status 1 -> B200MPI_ERR_TIMEOUT).
+// sync_end still runs, so nobody hangs, and no buffer is touched.
+// The signature covers the grid size.  CTAs other than 0 first look at what every peer's CTA 0
+// announced (slot row 0 of this rank's heap): if the peers launched a different grid, a CTA
+// without a partner learns it there instead of waiting for a flag that never comes.  (While the
+// grids match the row cannot be overwritten early: a peer's next kernel starts only after its
+// current one has finished, which needs this CTA to have passed sync_end.)
 __device__ __forceinline__ bool sync_start(const Comm& c, uint64_t a, uint64_t b, uint64_t* s_a,
                                            uint64_t* s_b) {
   int* verdict = start_verdict();
@@ -231,15 +250,7 @@ __device__ __forceinline__ bool sync_start(const Comm& c, uint64_t a, uint64_t b
     }
   }
   __syncthreads();
-  const int v = *verdict;
-  if (v) {
-    if (t == 0 && v != 3) { // a watchdog expiry has already raised status 1
-      *(volatile uint32_t*)c.status = 2u;
-      __threadfence_system();
-    }
-    return false;
-  }
-  return true;
+  return start_agreed(c);
 }
 
 // The start barrier of a call whose ranks hold different tables (Alltoallv).  Thread t announces
@@ -286,15 +297,7 @@ __device__ __forceinline__ bool sync_start_pairs(const Comm& c, uint64_t base_si
   __syncthreads();
   if (t == 0 && *verdict == 0 && sums[1] != want_sum) *verdict = 1;
   __syncthreads();
-  const int v = *verdict;
-  if (v) {
-    if (t == 0 && v != 3) {
-      *(volatile uint32_t*)c.status = 2u;
-      __threadfence_system();
-    }
-    return false;
-  }
-  return true;
+  return start_agreed(c);
 }
 
 // Per-CTA barrier #2: all of this CTA's stores (local, peer and multicast) are released to every
@@ -333,6 +336,21 @@ __device__ __forceinline__ void sync_mid(const Comm& c, uint32_t value) {
     wait_flag(&slot_of(c, c.rank, blockIdx.x, t)->flag, value, c);
   }
   __syncthreads();
+}
+
+// The frame of a collective kernel: sync_start announcing this rank's offsets a and b, then
+// body(s_a, s_b) with every rank's offsets, then sync_end.  A refused call skips the body and leaves
+// through sync_end_failed.  A CTA that left any other way would keep its peers waiting until the
+// watchdog fires, so every kernel of that shape goes through here.
+template <typename Body>
+__device__ __forceinline__ void collective(const Comm& c, uint64_t a, uint64_t b, Body body) {
+  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
+  if (!sync_start(c, a, b, s_a, s_b)) { // ranks disagree about this call: touch nothing, leave through the end barrier
+    sync_end_failed(c);
+    return;
+  }
+  body(s_a, s_b);
+  sync_end(c);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -411,6 +429,64 @@ __device__ __forceinline__ bool all_aligned16(const uint64_t* s_a, const uint64_
   return (m & 15) == 0;
 }
 
+// Element e of the n buffers at byte addresses src(0), ..., src(n-1), reduced in rank order:
+// acc = x_0; acc = op(acc, x_r) for r = 1..n-1.
+template <typename T, typename Op, typename Src>
+__device__ __forceinline__ T reduce_ranks(Src src, int n, size_t e) {
+  T acc = reinterpret_cast<const volatile T*>(src(0))[e];
+  for (int r = 1; r < n; ++r) acc = Op::template apply<T>(acc, reinterpret_cast<const volatile T*>(src(r))[e]);
+  return acc;
+}
+// ... of the n sends of a call (rank r's at heap offset s_a[r])
+template <typename T, typename Op>
+__device__ __forceinline__ T reduce_ranks(const Comm& c, const uint64_t* s_a, int n, size_t e) {
+  return reduce_ranks<T, Op>([&](int r) { return c.base[r] + s_a[r]; }, n, e);
+}
+
+// Elements [lo, hi), CTA bid of nb working on them: each reduced over the n sends in rank order and
+// stored, one element at a time, into every rank's recv (only_dst < 0) or into rank only_dst's.
+template <typename T, typename Op>
+__device__ __forceinline__ void reduce_store_elements(const Comm& c, const uint64_t* s_a, const uint64_t* s_b, int n, size_t lo, size_t hi,
+                                                      unsigned bid, unsigned nb, int only_dst = -1) {
+  const size_t gtid = (size_t)bid * blockDim.x + threadIdx.x;
+  for (size_t e = lo + gtid; e < hi; e += (size_t)nb * blockDim.x) {
+    const T acc = reduce_ranks<T, Op>(c, s_a, n, e);
+    for (int r = 0; r < n; ++r)
+      if (only_dst < 0 || r == only_dst) reinterpret_cast<volatile T*>(c.base[r] + s_b[r])[e] = acc;
+  }
+}
+
+// Rank `rank`'s contiguous share [lo, hi) of `count` elements cut into n equal parts (the last ones
+// may be short or empty): element ownership of unaligned buffers.
+struct Range {
+  size_t lo, hi;
+};
+__device__ __forceinline__ Range owned_elements(size_t count, int n, int rank) {
+  const size_t per = (count + n - 1) / n;
+  const size_t lo = per * rank < count ? per * rank : count;
+  return {lo, lo + per < count ? lo + per : count};
+}
+
+// The grid-strided copy loop of units [lo, hi): each thread loads UNROLL units (load(i, v)) before it
+// stores any of them (store(i, v)), so UNROLL loads are in flight per thread.
+template <int UNROLL, typename V, typename Load, typename Store>
+__device__ __forceinline__ void unrolled(size_t lo, size_t hi, Load load, Store store) {
+  const size_t step = (size_t)gridDim.x * blockDim.x * UNROLL;
+  for (size_t i0 = lo + (size_t)blockIdx.x * blockDim.x * UNROLL + threadIdx.x; i0 < hi; i0 += step) {
+    V v[UNROLL];
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u) {
+      const size_t i = i0 + (size_t)u * blockDim.x;
+      if (i < hi) load(i, v[u]);
+    }
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u) {
+      const size_t i = i0 + (size_t)u * blockDim.x;
+      if (i < hi) store(i, v[u]);
+    }
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // Allreduce, one-shot: every rank reads all n buffers and keeps the whole result (latency path).
 // The work is cut into rounds of one unit per thread.  When any rank runs in place
@@ -426,49 +502,41 @@ __device__ __forceinline__ bool any_inplace(const uint64_t* s_a, const uint64_t*
 template <typename T, typename Op, int NR>
 __global__ void __launch_bounds__(kThreads, 1)
 allreduce_oneshot_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t count) {
-  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
-  const bool call_ok = sync_start(c, send_off, recv_off, s_a, s_b);
-  if (!call_ok) { // ranks disagree about this call: touch nothing, leave through the end barrier
-    sync_end_failed(c);
-    return;
-  }
-  const int n = NR ? NR : c.n;
-  const size_t gtid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t gstride = (size_t)gridDim.x * blockDim.x;
-  char* out = c.base[c.rank] + s_b[c.rank];
-  const bool inplace = any_inplace(s_a, s_b, n);
-  uint32_t mid = c.epoch + 1;
-  constexpr int EPV = Pack<T>::N;
-  const bool al = all_aligned16(s_a, s_b, n);
-  const size_t nvec = al ? count / EPV : 0;
-  for (size_t base = 0; base < nvec; base += gstride) {
-    const size_t i = base + gtid;
-    Pack<T> acc;
-    if (i < nvec) {
-      Pack<T> v[NR ? NR : kMaxRanks];
+  collective(c, send_off, recv_off, [&](const uint64_t* s_a, const uint64_t* s_b) {
+    const int n = NR ? NR : c.n;
+    const size_t gtid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const size_t gstride = (size_t)gridDim.x * blockDim.x;
+    char* out = c.base[c.rank] + s_b[c.rank];
+    const bool inplace = any_inplace(s_a, s_b, n);
+    uint32_t mid = c.epoch + 1;
+    constexpr int EPV = Pack<T>::N;
+    const bool al = all_aligned16(s_a, s_b, n);
+    const size_t nvec = al ? count / EPV : 0;
+    for (size_t base = 0; base < nvec; base += gstride) {
+      const size_t i = base + gtid;
+      Pack<T> acc;
+      if (i < nvec) {
+        Pack<T> v[NR ? NR : kMaxRanks];
 #pragma unroll
-      for (int r = 0; r < (NR ? NR : kMaxRanks); ++r)
-        if (r < n) v[r] = ld_pack<T>(c.base[r] + s_a[r] + i * 16);
-      acc = v[0];
+        for (int r = 0; r < (NR ? NR : kMaxRanks); ++r)
+          if (r < n) v[r] = ld_pack<T>(c.base[r] + s_a[r] + i * 16);
+        acc = v[0];
 #pragma unroll
-      for (int r = 1; r < (NR ? NR : kMaxRanks); ++r)
-        if (r < n) acc = combine<T, Op>(acc, v[r]);
+        for (int r = 1; r < (NR ? NR : kMaxRanks); ++r)
+          if (r < n) acc = combine<T, Op>(acc, v[r]);
+      }
+      if (inplace) sync_mid(c, mid++);
+      if (i < nvec) st_pack<T>(out + i * 16, acc);
     }
-    if (inplace) sync_mid(c, mid++);
-    if (i < nvec) st_pack<T>(out + i * 16, acc);
-  }
-  // scalar rounds: the count % EPV tail, or everything when some buffer is not 16-byte aligned
-  for (size_t base = nvec * EPV; base < count; base += gstride) {
-    const size_t e = base + gtid;
-    T acc = T(0);
-    if (e < count) {
-      acc = reinterpret_cast<const volatile T*>(c.base[0] + s_a[0])[e];
-      for (int r = 1; r < n; ++r) acc = Op::template apply<T>(acc, reinterpret_cast<const volatile T*>(c.base[r] + s_a[r])[e]);
+    // scalar rounds: the count % EPV tail, or everything when some buffer is not 16-byte aligned
+    for (size_t base = nvec * EPV; base < count; base += gstride) {
+      const size_t e = base + gtid;
+      T acc = T(0);
+      if (e < count) acc = reduce_ranks<T, Op>(c, s_a, n, e);
+      if (inplace) sync_mid(c, mid++);
+      if (e < count) reinterpret_cast<T*>(out)[e] = acc;
     }
-    if (inplace) sync_mid(c, mid++);
-    if (e < count) reinterpret_cast<T*>(out)[e] = acc;
-  }
-  sync_end(c);
+  });
 }
 
 // One-shot with a lane per peer and warp-shuffle partial sums (n = 2, 4, 8; tree order).
@@ -477,63 +545,58 @@ allreduce_oneshot_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t co
 template <typename T, typename Op, int NR>
 __global__ void __launch_bounds__(kThreads, 1)
 allreduce_oneshot_shfl_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t count) {
-  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
   __shared__ const char* s_src[kMaxRanks];
-  const bool call_ok = sync_start(c, send_off, recv_off, s_a, s_b);
-  if (!call_ok) { // ranks disagree about this call: touch nothing, leave through the end barrier
-    sync_end_failed(c);
-    return;
-  }
-  if (threadIdx.x < NR) s_src[threadIdx.x] = c.base[threadIdx.x] + s_a[threadIdx.x];
-  __syncthreads();
-  constexpr int EPV = Pack<T>::N;
-  constexpr int VPW = 32 / NR; // vectors per warp step
-  const int lane = threadIdx.x & 31;
-  const int peer = lane % NR, sub = lane / NR;
-  const size_t warp = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const size_t nwarps = ((size_t)gridDim.x * blockDim.x) >> 5;
-  char* out = c.base[c.rank] + s_b[c.rank];
-  const bool al = all_aligned16(s_a, s_b, NR);
-  const bool inplace = any_inplace(s_a, s_b, NR);
-  uint32_t mid = c.epoch + 1;
-  const size_t nvec = al ? count / EPV : 0;
-  const char* src = s_src[peer];
-  for (size_t round = 0; round < nvec; round += nwarps * VPW) { // uniform across the CTA
-    const size_t i = round + warp * VPW + sub;
-    const bool valid = i < nvec;
-    Pack<T> v;
-    if (valid) v = ld_pack<T>(src + i * 16);
-    else
-      for (int k = 0; k < EPV; ++k) v.v[k] = T(0);
+  collective(c, send_off, recv_off, [&](const uint64_t* s_a, const uint64_t* s_b) {
+    if (threadIdx.x < NR) s_src[threadIdx.x] = c.base[threadIdx.x] + s_a[threadIdx.x];
+    __syncthreads();
+    constexpr int EPV = Pack<T>::N;
+    constexpr int VPW = 32 / NR; // vectors per warp step
+    const int lane = threadIdx.x & 31;
+    const int peer = lane % NR, sub = lane / NR;
+    const size_t warp = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const size_t nwarps = ((size_t)gridDim.x * blockDim.x) >> 5;
+    char* out = c.base[c.rank] + s_b[c.rank];
+    const bool al = all_aligned16(s_a, s_b, NR);
+    const bool inplace = any_inplace(s_a, s_b, NR);
+    uint32_t mid = c.epoch + 1;
+    const size_t nvec = al ? count / EPV : 0;
+    const char* src = s_src[peer];
+    for (size_t round = 0; round < nvec; round += nwarps * VPW) { // uniform across the CTA
+      const size_t i = round + warp * VPW + sub;
+      const bool valid = i < nvec;
+      Pack<T> v;
+      if (valid) v = ld_pack<T>(src + i * 16);
+      else
+        for (int k = 0; k < EPV; ++k) v.v[k] = T(0);
 #pragma unroll
-    for (int m = 1; m < NR; m <<= 1) {
-      union { Pack<T> k; uint32_t w[4]; } a, b;
-      a.k = v;
+      for (int m = 1; m < NR; m <<= 1) {
+        union { Pack<T> k; uint32_t w[4]; } a, b;
+        a.k = v;
 #pragma unroll
-      for (int w = 0; w < 4; ++w) b.w[w] = __shfl_xor_sync(0xffffffffu, a.w[w], m);
-      v = (peer & m) ? combine<T, Op>(b.k, v) : combine<T, Op>(v, b.k); // lower ranks on the left
+        for (int w = 0; w < 4; ++w) b.w[w] = __shfl_xor_sync(0xffffffffu, a.w[w], m);
+        v = (peer & m) ? combine<T, Op>(b.k, v) : combine<T, Op>(v, b.k); // lower ranks on the left
+      }
+      if (inplace) sync_mid(c, mid++);
+      if (peer == 0 && valid) st_pack<T>(out + i * 16, v);
     }
-    if (inplace) sync_mid(c, mid++);
-    if (peer == 0 && valid) st_pack<T>(out + i * 16, v);
-  }
-  // scalar rounds (tail, or the whole message when unaligned), tree order too
-  const size_t gtid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t gstride = (size_t)gridDim.x * blockDim.x;
-  for (size_t base = nvec * EPV; base < count; base += gstride) {
-    const size_t e = base + gtid;
-    T x[NR];
-    if (e < count) {
+    // scalar rounds (tail, or the whole message when unaligned), tree order too
+    const size_t gtid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const size_t gstride = (size_t)gridDim.x * blockDim.x;
+    for (size_t base = nvec * EPV; base < count; base += gstride) {
+      const size_t e = base + gtid;
+      T x[NR];
+      if (e < count) {
 #pragma unroll
-      for (int r = 0; r < NR; ++r) x[r] = reinterpret_cast<const volatile T*>(s_src[r])[e];
+        for (int r = 0; r < NR; ++r) x[r] = reinterpret_cast<const volatile T*>(s_src[r])[e];
 #pragma unroll
-      for (int m = 1; m < NR; m <<= 1)
+        for (int m = 1; m < NR; m <<= 1)
 #pragma unroll
-        for (int r = 0; r < NR; r += 2 * m) x[r] = Op::template apply<T>(x[r], x[r + m]);
+          for (int r = 0; r < NR; r += 2 * m) x[r] = Op::template apply<T>(x[r], x[r + m]);
+      }
+      if (inplace) sync_mid(c, mid++);
+      if (e < count) reinterpret_cast<T*>(out)[e] = x[0];
     }
-    if (inplace) sync_mid(c, mid++);
-    if (e < count) reinterpret_cast<T*>(out)[e] = x[0];
-  }
-  sync_end(c);
+  });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -560,6 +623,28 @@ struct Owner {
     return ((q * n + rank) << shift) + w;
   }
 };
+
+// `unrolled` over this rank's local slots, CTA bid of nb working on them: each thread loads the
+// vectors g < own.nvec of UNROLL slots (load(g, v)) before it stores any of them (store(g, v)).
+// twoshot_body, scan_kernel and nvls_body keep this loop written out: through the helper they
+// compiled to different SASS.
+template <int UNROLL, typename V, typename Load, typename Store>
+__device__ __forceinline__ void unrolled_owned(const Owner& own, unsigned bid, unsigned nb, Load load, Store store) {
+  const size_t step = (size_t)nb * blockDim.x * UNROLL;
+  for (size_t l0 = (size_t)bid * blockDim.x * UNROLL + threadIdx.x; l0 < own.slots; l0 += step) {
+    V v[UNROLL];
+    size_t gi[UNROLL];
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u) {
+      const size_t l = l0 + (size_t)u * blockDim.x;
+      gi[u] = l < own.slots ? own.global(l) : own.nvec;
+      if (gi[u] < own.nvec) load(gi[u], v[u]);
+    }
+#pragma unroll
+    for (int u = 0; u < UNROLL; ++u)
+      if (gi[u] < own.nvec) store(gi[u], v[u]);
+  }
+}
 
 // ---------------------------------------------------------------------------------------------
 // Allreduce, two-shot fused in one pass: the owner of a vector loads it from all n ranks
@@ -623,40 +708,20 @@ __device__ __forceinline__ void twoshot_body(const Comm& c, const uint64_t* s_a,
       }
     }
     // elements past the last whole vector: reduced and pushed by the last rank
-    if (c.rank == n - 1) {
-      const size_t gtid = (size_t)bid * blockDim.x + tid;
-      for (size_t e = nvec * EPV + gtid; e < count; e += (size_t)nb * blockDim.x) {
-        T acc = reinterpret_cast<const volatile T*>(c.base[0] + s_a[0])[e];
-        for (int r = 1; r < n; ++r) acc = Op::template apply<T>(acc, reinterpret_cast<const volatile T*>(c.base[r] + s_a[r])[e]);
-        for (int r = 0; r < n; ++r)
-          if (only_dst < 0 || r == only_dst) reinterpret_cast<volatile T*>(c.base[r] + s_b[r])[e] = acc;
-      }
-    }
+    if (c.rank == n - 1) reduce_store_elements<T, Op>(c, s_a, s_b, n, nvec * EPV, count, bid, nb, only_dst);
   } else {
     // unaligned buffers: contiguous ownership by element, scalar accesses
-    const size_t per = (count + n - 1) / n;
-    const size_t lo = per * c.rank < count ? per * c.rank : count;
-    const size_t hi = lo + per < count ? lo + per : count;
-    for (size_t e = lo + (size_t)bid * blockDim.x + tid; e < hi; e += (size_t)nb * blockDim.x) {
-      T acc = reinterpret_cast<const volatile T*>(c.base[0] + s_a[0])[e];
-      for (int r = 1; r < n; ++r) acc = Op::template apply<T>(acc, reinterpret_cast<const volatile T*>(c.base[r] + s_a[r])[e]);
-      for (int r = 0; r < n; ++r)
-        if (only_dst < 0 || r == only_dst) reinterpret_cast<volatile T*>(c.base[r] + s_b[r])[e] = acc;
-    }
+    const Range mine = owned_elements(count, n, c.rank);
+    reduce_store_elements<T, Op>(c, s_a, s_b, n, mine.lo, mine.hi, bid, nb, only_dst);
   }
 }
 
 template <typename T, typename Op, int NR, int UNROLL>
 __global__ void __launch_bounds__(kThreads, 1)
 allreduce_twoshot_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t count, uint32_t shift, int only_dst) {
-  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
-  const bool call_ok = sync_start(c, send_off, recv_off, s_a, s_b);
-  if (!call_ok) { // ranks disagree about this call: touch nothing, leave through the end barrier
-    sync_end_failed(c);
-    return;
-  }
-  twoshot_body<T, Op, NR, UNROLL>(c, s_a, s_b, count, shift, blockIdx.x, gridDim.x, only_dst);
-  sync_end(c);
+  collective(c, send_off, recv_off, [&](const uint64_t* s_a, const uint64_t* s_b) {
+    twoshot_body<T, Op, NR, UNROLL>(c, s_a, s_b, count, shift, blockIdx.x, gridDim.x, only_dst);
+  });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -690,70 +755,63 @@ __device__ __forceinline__ void scan_element(const Comm& c, const uint64_t* s_a,
 template <typename T, typename Op, int NR, int UNROLL, bool EXCLUSIVE>
 __global__ void __launch_bounds__(kThreads, 1)
 scan_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t count, uint32_t shift) {
-  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
-  const bool call_ok = sync_start(c, send_off, recv_off, s_a, s_b);
-  if (!call_ok) { // ranks disagree about this call: touch nothing, leave through the end barrier
-    sync_end_failed(c);
-    return;
-  }
-  const int n = NR ? NR : c.n;
-  const int nin = EXCLUSIVE ? n - 1 : n; // ranks whose input any result needs
-  constexpr int R = NR ? NR : kMaxRanks;
-  constexpr int EPV = Pack<T>::N;
-  const size_t tid = threadIdx.x;
-  const size_t nthreads = (size_t)gridDim.x * blockDim.x;
-  if (all_aligned16(s_a, s_b, n)) {
-    const size_t nvec = count / EPV;
-    const Owner own(nvec, shift, n, c.rank);
-    __shared__ const char* src[kMaxRanks];
-    __shared__ char* dst[kMaxRanks];
-    if (tid < (size_t)R) {
-      const int r = (int)tid < n ? (int)tid : 0;
-      src[tid] = c.base[r] + s_a[r];
-      dst[tid] = c.base[r] + s_b[r];
-    }
-    __syncthreads();
-    const size_t step = nthreads * UNROLL;
-    for (size_t l0 = (size_t)blockIdx.x * blockDim.x * UNROLL + tid; l0 < own.slots; l0 += step) {
-      Pack<T> v[UNROLL][R];
-      size_t gi[UNROLL];
+  __shared__ const char* src[kMaxRanks];
+  __shared__ char* dst[kMaxRanks];
+  collective(c, send_off, recv_off, [&](const uint64_t* s_a, const uint64_t* s_b) {
+    const int n = NR ? NR : c.n;
+    const int nin = EXCLUSIVE ? n - 1 : n; // ranks whose input any result needs
+    constexpr int R = NR ? NR : kMaxRanks;
+    constexpr int EPV = Pack<T>::N;
+    const size_t tid = threadIdx.x;
+    const size_t nthreads = (size_t)gridDim.x * blockDim.x;
+    if (all_aligned16(s_a, s_b, n)) {
+      const size_t nvec = count / EPV;
+      const Owner own(nvec, shift, n, c.rank);
+      if (tid < (size_t)R) {
+        const int r = (int)tid < n ? (int)tid : 0;
+        src[tid] = c.base[r] + s_a[r];
+        dst[tid] = c.base[r] + s_b[r];
+      }
+      __syncthreads();
+      const size_t step = nthreads * UNROLL;
+      for (size_t l0 = (size_t)blockIdx.x * blockDim.x * UNROLL + tid; l0 < own.slots; l0 += step) {
+        Pack<T> v[UNROLL][R];
+        size_t gi[UNROLL];
 #pragma unroll
-      for (int u = 0; u < UNROLL; ++u) {
-        const size_t l = l0 + (size_t)u * blockDim.x;
-        gi[u] = l < own.slots ? own.global(l) : nvec;
-        if (gi[u] < nvec) {
+        for (int u = 0; u < UNROLL; ++u) {
+          const size_t l = l0 + (size_t)u * blockDim.x;
+          gi[u] = l < own.slots ? own.global(l) : nvec;
+          if (gi[u] < nvec) {
 #pragma unroll
-          for (int r = 0; r < R; ++r)
-            if (r < nin) v[u][r] = ld_pack<T>(src[r] + gi[u] * 16);
+            for (int r = 0; r < R; ++r)
+              if (r < nin) v[u][r] = ld_pack<T>(src[r] + gi[u] * 16);
+          }
+        }
+#pragma unroll
+        for (int u = 0; u < UNROLL; ++u) {
+          if (gi[u] < nvec) {
+#pragma unroll
+            for (int r = 1; r < R; ++r) // v[u][r] becomes prefix r
+              if (r < nin) v[u][r] = combine<T, Op>(v[u][r - 1], v[u][r]);
+            // rank r's result is prefix r (Scan) or prefix r-1 (Exscan); ranks after this one first
+#pragma unroll
+            for (int r = EXCLUSIVE ? 1 : 0; r < R; ++r)
+              if (r > c.rank && r < n) st_pack<T>(dst[r] + gi[u] * 16, v[u][EXCLUSIVE ? r - 1 : r]);
+#pragma unroll
+            for (int r = EXCLUSIVE ? 1 : 0; r < R; ++r)
+              if (r <= c.rank) st_pack<T>(dst[r] + gi[u] * 16, v[u][EXCLUSIVE ? r - 1 : r]);
+          }
         }
       }
-#pragma unroll
-      for (int u = 0; u < UNROLL; ++u) {
-        if (gi[u] < nvec) {
-#pragma unroll
-          for (int r = 1; r < R; ++r) // v[u][r] becomes prefix r
-            if (r < nin) v[u][r] = combine<T, Op>(v[u][r - 1], v[u][r]);
-          // rank r's result is prefix r (Scan) or prefix r-1 (Exscan); ranks after this one first
-#pragma unroll
-          for (int r = EXCLUSIVE ? 1 : 0; r < R; ++r)
-            if (r > c.rank && r < n) st_pack<T>(dst[r] + gi[u] * 16, v[u][EXCLUSIVE ? r - 1 : r]);
-#pragma unroll
-          for (int r = EXCLUSIVE ? 1 : 0; r < R; ++r)
-            if (r <= c.rank) st_pack<T>(dst[r] + gi[u] * 16, v[u][EXCLUSIVE ? r - 1 : r]);
-        }
-      }
+      // elements past the last whole vector: reduced and pushed by the last rank
+      if (c.rank == n - 1)
+        for (size_t e = nvec * EPV + (size_t)blockIdx.x * blockDim.x + tid; e < count; e += nthreads) scan_element<T, Op, EXCLUSIVE>(c, s_a, s_b, n, e);
+    } else {
+      // unaligned buffers: contiguous ownership by element, scalar accesses
+      const Range mine = owned_elements(count, n, c.rank);
+      for (size_t e = mine.lo + (size_t)blockIdx.x * blockDim.x + tid; e < mine.hi; e += nthreads) scan_element<T, Op, EXCLUSIVE>(c, s_a, s_b, n, e);
     }
-    // elements past the last whole vector: reduced and pushed by the last rank
-    if (c.rank == n - 1)
-      for (size_t e = nvec * EPV + (size_t)blockIdx.x * blockDim.x + tid; e < count; e += nthreads) scan_element<T, Op, EXCLUSIVE>(c, s_a, s_b, n, e);
-  } else {
-    // unaligned buffers: contiguous ownership by element, scalar accesses
-    const size_t per = (count + n - 1) / n;
-    const size_t lo = per * c.rank < count ? per * c.rank : count;
-    const size_t hi = lo + per < count ? lo + per : count;
-    for (size_t e = lo + (size_t)blockIdx.x * blockDim.x + tid; e < hi; e += nthreads) scan_element<T, Op, EXCLUSIVE>(c, s_a, s_b, n, e);
-  }
-  sync_end(c);
+  });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -807,105 +865,92 @@ template <typename T, typename Op, int NR>
 __global__ void __launch_bounds__(kSmemThreads, 1)
 allreduce_twoshot_smem_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t count, uint32_t shift) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
   __shared__ __align__(8) uint64_t full_bar[kSmemStages], empty_bar[kSmemStages];
-  unsigned char* in_tiles = smem_raw;                                         // [stage][rank][chunk]
-  unsigned char* out_tiles = smem_raw + (size_t)kSmemStages * NR * kSmemChunk; // [ostage][chunk]
-  const bool call_ok = sync_start(c, send_off, recv_off, s_a, s_b);
-  if (!call_ok) { // ranks disagree about this call: touch nothing, leave through the end barrier
-    sync_end_failed(c);
-    return;
-  }
-  constexpr int EPV = Pack<T>::N;
-  const int tid = threadIdx.x;
-  const bool al = all_aligned16(s_a, s_b, NR);
-  const size_t nvec = al ? count / EPV : 0;
-  // shift >= 8 (a block is a whole number of 4 KiB tiles); tile t covers local slots [t*256, t*256+256)
-  const Owner own(nvec, shift, NR, c.rank);
-  constexpr size_t kTileVecs = kSmemChunk / 16;
-  const size_t ntiles = own.slots / kTileVecs;
-  if (tid == 0) {
-    for (int s = 0; s < kSmemStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], kSmemConsumers / 32);
+  collective(c, send_off, recv_off, [&](const uint64_t* s_a, const uint64_t* s_b) {
+    unsigned char* in_tiles = smem_raw;                                         // [stage][rank][chunk]
+    unsigned char* out_tiles = smem_raw + (size_t)kSmemStages * NR * kSmemChunk; // [ostage][chunk]
+    constexpr int EPV = Pack<T>::N;
+    const int tid = threadIdx.x;
+    const bool al = all_aligned16(s_a, s_b, NR);
+    const size_t nvec = al ? count / EPV : 0;
+    // shift >= 8 (a block is a whole number of 4 KiB tiles); tile t covers local slots [t*256, t*256+256)
+    const Owner own(nvec, shift, NR, c.rank);
+    constexpr size_t kTileVecs = kSmemChunk / 16;
+    const size_t ntiles = own.slots / kTileVecs;
+    if (tid == 0) {
+      for (int s = 0; s < kSmemStages; ++s) {
+        mbar_init(&full_bar[s], 1);
+        mbar_init(&empty_bar[s], kSmemConsumers / 32);
+      }
+      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  if (tid >= kSmemConsumers) {
-    // ---- producer warp: one lane drives the TMA loads ----
-    if (tid == kSmemConsumers) {
-      uint32_t it = 0;
-      for (size_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
-        if (own.global(t * kTileVecs) >= nvec) continue;
-        const int s = it % kSmemStages;
-        const uint32_t use = it / kSmemStages;
-        ++it;
-        if (use > 0) mbar_wait(&empty_bar[s], (use - 1) & 1);
-        const size_t g0 = own.global(t * kTileVecs);
-        const size_t off = g0 * 16;
-        const uint32_t bytes = (uint32_t)((nvec - g0) < kTileVecs ? (nvec - g0) * 16 : (size_t)kSmemChunk);
-        mbar_expect_tx(&full_bar[s], bytes * NR);
+    __syncthreads();
+    if (tid >= kSmemConsumers) {
+      // ---- producer warp: one lane drives the TMA loads ----
+      if (tid == kSmemConsumers) {
+        uint32_t it = 0;
+        for (size_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
+          if (own.global(t * kTileVecs) >= nvec) continue;
+          const int s = it % kSmemStages;
+          const uint32_t use = it / kSmemStages;
+          ++it;
+          if (use > 0) mbar_wait(&empty_bar[s], (use - 1) & 1);
+          const size_t g0 = own.global(t * kTileVecs);
+          const size_t off = g0 * 16;
+          const uint32_t bytes = (uint32_t)((nvec - g0) < kTileVecs ? (nvec - g0) * 16 : (size_t)kSmemChunk);
+          mbar_expect_tx(&full_bar[s], bytes * NR);
 #pragma unroll
-        for (int r = 0; r < NR; ++r)
-          bulk_g2s(in_tiles + ((size_t)s * NR + r) * kSmemChunk, c.base[r] + s_a[r] + off, bytes, &full_bar[s]);
-      }
-    }
-  } else {
-    // ---- consumer warps ----
-    uint32_t nit = 0;
-    for (size_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
-      const size_t g0 = own.global(t * kTileVecs);
-      if (g0 >= nvec) continue;
-      const uint32_t it = nit++;
-      const int s = it % kSmemStages;
-      const int os = it % kSmemOutStages;
-      const uint32_t bytes = (uint32_t)((nvec - g0) < kTileVecs ? (nvec - g0) * 16 : (size_t)kSmemChunk);
-      mbar_wait(&full_bar[s], (it / kSmemStages) & 1);
-      if (it >= (uint32_t)kSmemOutStages) { // the stores that read out_tiles[os] two tiles ago must have drained it
-        if (tid == 0) bulk_wait_read<kSmemOutStages - 1>();
-        asm volatile("bar.sync 1, %0;" ::"n"(kSmemConsumers) : "memory");
-      }
-      if ((uint32_t)tid * 16 < bytes) {
-        const unsigned char* src = in_tiles + (size_t)s * NR * kSmemChunk + (size_t)tid * 16;
-        Pack<T> acc = *reinterpret_cast<const Pack<T>*>(src);
-#pragma unroll
-        for (int r = 1; r < NR; ++r) acc = combine<T, Op>(acc, *reinterpret_cast<const Pack<T>*>(src + (size_t)r * kSmemChunk));
-        *reinterpret_cast<Pack<T>*>(out_tiles + (size_t)os * kSmemChunk + (size_t)tid * 16) = acc;
-      }
-      fence_proxy_async_smem(); // generic-proxy writes to out_tiles -> visible to the bulk-copy engine
-      asm volatile("bar.sync 1, %0;" ::"n"(kSmemConsumers) : "memory");
-      if ((tid & 31) == 0) mbar_arrive(&empty_bar[s]); // this warp is done reading in_tiles[s]
-      if (tid == 0) {
-        const size_t off = g0 * 16;
-#pragma unroll
-        for (int r = 0; r < NR; ++r) {
-          const int w = (c.rank + 1 + r) % NR;
-          bulk_s2g(c.base[w] + s_b[w] + off, out_tiles + (size_t)os * kSmemChunk, bytes);
+          for (int r = 0; r < NR; ++r)
+            bulk_g2s(in_tiles + ((size_t)s * NR + r) * kSmemChunk, c.base[r] + s_a[r] + off, bytes, &full_bar[s]);
         }
-        bulk_commit();
       }
+    } else {
+      // ---- consumer warps ----
+      uint32_t nit = 0;
+      for (size_t t = blockIdx.x; t < ntiles; t += gridDim.x) {
+        const size_t g0 = own.global(t * kTileVecs);
+        if (g0 >= nvec) continue;
+        const uint32_t it = nit++;
+        const int s = it % kSmemStages;
+        const int os = it % kSmemOutStages;
+        const uint32_t bytes = (uint32_t)((nvec - g0) < kTileVecs ? (nvec - g0) * 16 : (size_t)kSmemChunk);
+        mbar_wait(&full_bar[s], (it / kSmemStages) & 1);
+        if (it >= (uint32_t)kSmemOutStages) { // the stores that read out_tiles[os] two tiles ago must have drained it
+          if (tid == 0) bulk_wait_read<kSmemOutStages - 1>();
+          asm volatile("bar.sync 1, %0;" ::"n"(kSmemConsumers) : "memory");
+        }
+        if ((uint32_t)tid * 16 < bytes) {
+          const unsigned char* src = in_tiles + (size_t)s * NR * kSmemChunk + (size_t)tid * 16;
+          Pack<T> acc = *reinterpret_cast<const Pack<T>*>(src);
+#pragma unroll
+          for (int r = 1; r < NR; ++r) acc = combine<T, Op>(acc, *reinterpret_cast<const Pack<T>*>(src + (size_t)r * kSmemChunk));
+          *reinterpret_cast<Pack<T>*>(out_tiles + (size_t)os * kSmemChunk + (size_t)tid * 16) = acc;
+        }
+        fence_proxy_async_smem(); // generic-proxy writes to out_tiles -> visible to the bulk-copy engine
+        asm volatile("bar.sync 1, %0;" ::"n"(kSmemConsumers) : "memory");
+        if ((tid & 31) == 0) mbar_arrive(&empty_bar[s]); // this warp is done reading in_tiles[s]
+        if (tid == 0) {
+          const size_t off = g0 * 16;
+#pragma unroll
+          for (int r = 0; r < NR; ++r) {
+            const int w = (c.rank + 1 + r) % NR;
+            bulk_s2g(c.base[w] + s_b[w] + off, out_tiles + (size_t)os * kSmemChunk, bytes);
+          }
+          bulk_commit();
+        }
+      }
+      if (tid == 0) bulk_wait<0>(); // every peer write of this CTA has been performed
     }
-    if (tid == 0) bulk_wait<0>(); // every peer write of this CTA has been performed
-  }
-  // elements outside whole 16-byte vectors, or everything when unaligned: scalar, last rank / by ownership
-  {
+    // elements outside whole 16-byte vectors, or everything when unaligned: scalar, last rank / by ownership
+    // (stored here, not through reduce_store_elements, which compiled to different SASS in this kernel)
     const size_t gtid = (size_t)blockIdx.x * blockDim.x + tid;
     const size_t gstride = (size_t)gridDim.x * blockDim.x;
-    size_t elo, ehi;
-    if (al) { elo = c.rank == NR - 1 ? nvec * EPV : count; ehi = count; }
-    else {
-      const size_t pe = (count + NR - 1) / NR;
-      elo = pe * c.rank < count ? pe * c.rank : count;
-      ehi = elo + pe < count ? elo + pe : count;
-    }
-    for (size_t e = elo + gtid; e < ehi; e += gstride) {
-      T acc = reinterpret_cast<const volatile T*>(c.base[0] + s_a[0])[e];
-      for (int r = 1; r < NR; ++r) acc = Op::template apply<T>(acc, reinterpret_cast<const volatile T*>(c.base[r] + s_a[r])[e]);
+    const Range scalar = al ? Range{c.rank == NR - 1 ? nvec * EPV : count, count} : owned_elements(count, NR, c.rank);
+    for (size_t e = scalar.lo + gtid; e < scalar.hi; e += gstride) {
+      const T acc = reduce_ranks<T, Op>(c, s_a, NR, e);
       for (int r = 0; r < NR; ++r) reinterpret_cast<volatile T*>(c.base[r] + s_b[r])[e] = acc;
     }
-  }
-  sync_end(c);
+  });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -950,6 +995,7 @@ allreduce_ring_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t count
       if (threadIdx.x == 0) wait_flag(ring_flag(c, r, blockIdx.x), fbase + (uint32_t)g, c);
       __syncthreads();
     }
+    // owned_elements(groups, n, chunk), written out: through the helper this kernel compiled to different SASS
     const size_t lo = per * chunk < groups ? per * chunk : groups;
     const size_t hi = lo + per < groups ? lo + per : groups;
     const char* in = (g == 0) ? prev_send : prev_recv;
@@ -975,10 +1021,7 @@ allreduce_ring_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t count
   // tail: at most EPV-1 elements, one per thread of CTA 0, kept in a register across the barrier
   const size_t te = groups * EPV + tid;
   T tail = T(0);
-  if (te < count) {
-    tail = reinterpret_cast<const volatile T*>(c.base[0] + s_a[0])[te];
-    for (int q = 1; q < n; ++q) tail = Op::template apply<T>(tail, reinterpret_cast<const volatile T*>(c.base[q] + s_a[q])[te]);
-  }
+  if (te < count) tail = reduce_ranks<T, Op>(c, s_a, n, te);
   sync_end(c);
   __syncthreads(); // sync_end's waits are done by threads 0..n-1 only
   // after the barrier nobody reads this rank's send buffer any more (in-place safe)
@@ -1071,20 +1114,6 @@ __device__ __forceinline__ void nvls_body(const Comm& c, uint64_t send_off, uint
   }
 }
 
-// count % EPV trailing elements of an aligned message: last rank, rank order, P2P.
-template <typename T, typename Op>
-__device__ __forceinline__ void tail_body(const Comm& c, const uint64_t* s_a, const uint64_t* s_b, size_t first, size_t count,
-                                          unsigned bid, unsigned nb, int only_dst = -1) {
-  const int n = c.n;
-  if (c.rank != n - 1) return;
-  for (size_t e = first + (size_t)bid * blockDim.x + threadIdx.x; e < count; e += (size_t)nb * blockDim.x) {
-    T acc = reinterpret_cast<const volatile T*>(c.base[0] + s_a[0])[e];
-    for (int r = 1; r < n; ++r) acc = Op::template apply<T>(acc, reinterpret_cast<const volatile T*>(c.base[r] + s_a[r])[e]);
-    for (int r = 0; r < n; ++r)
-      if (only_dst < 0 || r == only_dst) reinterpret_cast<volatile T*>(c.base[r] + s_b[r])[e] = acc;
-  }
-}
-
 __device__ __forceinline__ bool symmetric_offsets(const uint64_t* s_a, const uint64_t* s_b, uint64_t send_off, uint64_t recv_off, int n) {
   bool sym = ((send_off | recv_off) & 15) == 0;
   for (int r = 0; r < n; ++r) sym = sym && s_a[r] == send_off && s_b[r] == recv_off;
@@ -1094,29 +1123,25 @@ __device__ __forceinline__ bool symmetric_offsets(const uint64_t* s_a, const uin
 template <typename T, typename Op, int UNROLL>
 __global__ void __launch_bounds__(kThreads, 1)
 allreduce_nvls_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t count, uint32_t shift, int only_dst) {
-  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
-  const bool call_ok = sync_start(c, send_off, recv_off, s_a, s_b);
-  if (!call_ok) { // ranks disagree about this call: touch nothing, leave through the end barrier
-    sync_end_failed(c);
-    return;
-  }
-  constexpr int EPV = Pack<T>::N;
-  // Reduce (only_dst >= 0): recv matters on the root only; the other ranks' recv offsets are ignored
-  bool symmetric;
-  if (only_dst < 0) symmetric = symmetric_offsets(s_a, s_b, send_off, recv_off, c.n);
-  else {
-    symmetric = ((send_off | s_b[only_dst]) & 15) == 0;
-    for (int r = 0; r < c.n; ++r) symmetric = symmetric && s_a[r] == send_off;
-  }
-  if (symmetric) {
-    const size_t nvec = count / EPV;
-    nvls_body<T, Op, UNROLL>(c, send_off, only_dst < 0 ? recv_off : s_b[only_dst], nvec, shift, blockIdx.x, gridDim.x, only_dst);
-    tail_body<T, Op>(c, s_a, s_b, nvec * EPV, count, blockIdx.x, gridDim.x, only_dst);
-  } else {
-    // the multicast address needs the same offsets on every rank; otherwise the P2P two-shot body
-    twoshot_body<T, Op, 0, 1>(c, s_a, s_b, count, shift, blockIdx.x, gridDim.x, only_dst);
-  }
-  sync_end(c);
+  collective(c, send_off, recv_off, [&](const uint64_t* s_a, const uint64_t* s_b) {
+    constexpr int EPV = Pack<T>::N;
+    // Reduce (only_dst >= 0): recv matters on the root only; the other ranks' recv offsets are ignored
+    bool symmetric;
+    if (only_dst < 0) symmetric = symmetric_offsets(s_a, s_b, send_off, recv_off, c.n);
+    else {
+      symmetric = ((send_off | s_b[only_dst]) & 15) == 0;
+      for (int r = 0; r < c.n; ++r) symmetric = symmetric && s_a[r] == send_off;
+    }
+    if (symmetric) {
+      const size_t nvec = count / EPV;
+      nvls_body<T, Op, UNROLL>(c, send_off, only_dst < 0 ? recv_off : s_b[only_dst], nvec, shift, blockIdx.x, gridDim.x, only_dst);
+      // count % EPV trailing elements: last rank, rank order, P2P
+      if (c.rank == c.n - 1) reduce_store_elements<T, Op>(c, s_a, s_b, c.n, nvec * EPV, count, blockIdx.x, gridDim.x, only_dst);
+    } else {
+      // the multicast address needs the same offsets on every rank; otherwise the P2P two-shot body
+      twoshot_body<T, Op, 0, 1>(c, s_a, s_b, count, shift, blockIdx.x, gridDim.x, only_dst);
+    }
+  });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1130,28 +1155,24 @@ template <typename T, typename Op, int NR, int UN, int UP>
 __global__ void __launch_bounds__(kThreads, 1)
 allreduce_hybrid_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t count, uint32_t shift_nvls, uint32_t shift_p2p,
                         size_t split_vec, unsigned nb_nvls) {
-  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks], s_a2[kMaxRanks], s_b2[kMaxRanks];
-  const bool call_ok = sync_start(c, send_off, recv_off, s_a, s_b);
-  if (!call_ok) {
-    sync_end_failed(c);
-    return;
-  }
-  constexpr int EPV = Pack<T>::N;
-  if (symmetric_offsets(s_a, s_b, send_off, recv_off, c.n)) {
-    if (blockIdx.x < nb_nvls) {
-      nvls_body<T, Op, UN>(c, send_off, recv_off, split_vec, shift_nvls, blockIdx.x, nb_nvls);
-    } else {
-      if (threadIdx.x < (unsigned)c.n) {
-        s_a2[threadIdx.x] = s_a[threadIdx.x] + split_vec * 16;
-        s_b2[threadIdx.x] = s_b[threadIdx.x] + split_vec * 16;
+  __shared__ uint64_t s_a2[kMaxRanks], s_b2[kMaxRanks];
+  collective(c, send_off, recv_off, [&](const uint64_t* s_a, const uint64_t* s_b) {
+    constexpr int EPV = Pack<T>::N;
+    if (symmetric_offsets(s_a, s_b, send_off, recv_off, c.n)) {
+      if (blockIdx.x < nb_nvls) {
+        nvls_body<T, Op, UN>(c, send_off, recv_off, split_vec, shift_nvls, blockIdx.x, nb_nvls);
+      } else {
+        if (threadIdx.x < (unsigned)c.n) {
+          s_a2[threadIdx.x] = s_a[threadIdx.x] + split_vec * 16;
+          s_b2[threadIdx.x] = s_b[threadIdx.x] + split_vec * 16;
+        }
+        __syncthreads();
+        twoshot_body<T, Op, NR, UP>(c, s_a2, s_b2, count - split_vec * EPV, shift_p2p, blockIdx.x - nb_nvls, gridDim.x - nb_nvls);
       }
-      __syncthreads();
-      twoshot_body<T, Op, NR, UP>(c, s_a2, s_b2, count - split_vec * EPV, shift_p2p, blockIdx.x - nb_nvls, gridDim.x - nb_nvls);
+    } else {
+      twoshot_body<T, Op, NR, UP>(c, s_a, s_b, count, shift_p2p, blockIdx.x, gridDim.x);
     }
-  } else {
-    twoshot_body<T, Op, NR, UP>(c, s_a, s_b, count, shift_p2p, blockIdx.x, gridDim.x);
-  }
-  sync_end(c);
+  });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1163,89 +1184,63 @@ allreduce_hybrid_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t cou
 template <typename T, typename Op, int UNROLL>
 __global__ void __launch_bounds__(kThreads, 1)
 reduce_scatter_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t count) {
-  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
-  __shared__ const char* src[kMaxRanks];
-  const bool call_ok = sync_start(c, send_off, recv_off, s_a, s_b);
-  if (!call_ok) {
-    sync_end_failed(c);
-    return;
-  }
-  const int n = c.n;
-  constexpr int EPV = Pack<T>::N;
-  const size_t blk_bytes = count * sizeof(T);
-  if (threadIdx.x < (unsigned)n) src[threadIdx.x] = c.base[threadIdx.x] + s_a[threadIdx.x] + (size_t)c.rank * blk_bytes;
-  __syncthreads();
-  char* out = c.base[c.rank] + recv_off;
-  uint64_t m = recv_off | blk_bytes; // block j of every rank must be 16-byte aligned for the vector path
-  for (int r = 0; r < n; ++r) m |= s_a[r];
-  const size_t nvec = (m & 15) == 0 ? count / EPV : 0;
-  const size_t tid = threadIdx.x;
-  const size_t step = (size_t)gridDim.x * blockDim.x * UNROLL;
-  for (size_t i0 = (size_t)blockIdx.x * blockDim.x * UNROLL + tid; i0 < nvec; i0 += step) {
-    Pack<T> acc[UNROLL];
-#pragma unroll
-    for (int u = 0; u < UNROLL; ++u) {
-      const size_t i = i0 + (size_t)u * blockDim.x;
-      if (i < nvec) {
-        acc[u] = ld_pack<T>(src[0] + i * 16);
-        for (int r = 1; r < n; ++r) acc[u] = combine<T, Op>(acc[u], ld_pack<T>(src[r] + i * 16));
-      }
-    }
-#pragma unroll
-    for (int u = 0; u < UNROLL; ++u) {
-      const size_t i = i0 + (size_t)u * blockDim.x;
-      if (i < nvec) st_pack<T>(out + i * 16, acc[u]);
-    }
-  }
-  for (size_t e = nvec * EPV + (size_t)blockIdx.x * blockDim.x + tid; e < count; e += (size_t)gridDim.x * blockDim.x) {
-    T acc = reinterpret_cast<const volatile T*>(src[0])[e];
-    for (int r = 1; r < n; ++r) acc = Op::template apply<T>(acc, reinterpret_cast<const volatile T*>(src[r])[e]);
-    reinterpret_cast<T*>(out)[e] = acc;
-  }
-  sync_end(c);
+  collective(c, send_off, recv_off, [&](const uint64_t* s_a, const uint64_t*) {
+    __shared__ const char* src[kMaxRanks];
+    const int n = c.n;
+    constexpr int EPV = Pack<T>::N;
+    const size_t blk_bytes = count * sizeof(T);
+    if (threadIdx.x < (unsigned)n) src[threadIdx.x] = c.base[threadIdx.x] + s_a[threadIdx.x] + (size_t)c.rank * blk_bytes;
+    __syncthreads();
+    char* out = c.base[c.rank] + recv_off;
+    uint64_t m = recv_off | blk_bytes; // block j of every rank must be 16-byte aligned for the vector path
+    for (int r = 0; r < n; ++r) m |= s_a[r];
+    const size_t nvec = (m & 15) == 0 ? count / EPV : 0;
+    unrolled<UNROLL, Pack<T>>(
+        0, nvec,
+        [&](size_t i, Pack<T>& acc) {
+          acc = ld_pack<T>(src[0] + i * 16);
+          for (int r = 1; r < n; ++r) acc = combine<T, Op>(acc, ld_pack<T>(src[r] + i * 16));
+        },
+        [&](size_t i, const Pack<T>& acc) { st_pack<T>(out + i * 16, acc); });
+    for (size_t e = nvec * EPV + (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < count; e += (size_t)gridDim.x * blockDim.x)
+      reinterpret_cast<T*>(out)[e] = reduce_ranks<T, Op>([&](int r) { return src[r]; }, n, e);
+  });
 }
 
 template <typename T, typename Op, int UNROLL>
 __global__ void __launch_bounds__(kThreads, 1)
 reduce_scatter_nvls_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t count) {
-  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
-  const bool call_ok = sync_start(c, send_off, recv_off, s_a, s_b);
-  if (!call_ok) {
-    sync_end_failed(c);
-    return;
-  }
-  const int n = c.n;
-  constexpr int EPV = Pack<T>::N;
-  const size_t blk_bytes = count * sizeof(T);
-  bool symmetric = ((send_off | recv_off | blk_bytes) & 15) == 0;
-  for (int r = 0; r < n; ++r) symmetric = symmetric && s_a[r] == send_off && (s_b[r] & 15) == 0;
-  char* out = c.base[c.rank] + recv_off;
-  const size_t tid = threadIdx.x;
-  if (symmetric) {
-    const size_t nvec = count / EPV; // blk_bytes % 16 == 0: no tail
-    const char* src = c.mc + send_off + (size_t)c.rank * blk_bytes;
-    const size_t step = (size_t)gridDim.x * blockDim.x * UNROLL;
-    for (size_t i0 = (size_t)blockIdx.x * blockDim.x * UNROLL + tid; i0 < nvec; i0 += step) {
-      Pack<T> v[UNROLL];
+  collective(c, send_off, recv_off, [&](const uint64_t* s_a, const uint64_t* s_b) {
+    const int n = c.n;
+    constexpr int EPV = Pack<T>::N;
+    const size_t blk_bytes = count * sizeof(T);
+    bool symmetric = ((send_off | recv_off | blk_bytes) & 15) == 0;
+    for (int r = 0; r < n; ++r) symmetric = symmetric && s_a[r] == send_off && (s_b[r] & 15) == 0;
+    char* out = c.base[c.rank] + recv_off;
+    const size_t tid = threadIdx.x;
+    if (symmetric) {
+      const char* src = c.mc + send_off + (size_t)c.rank * blk_bytes;
+      // written out: through `unrolled` this loop compiled to different SASS (+1 register for f64)
+      const size_t nvec = count / EPV; // blk_bytes % 16 == 0: no tail
+      const size_t step = (size_t)gridDim.x * blockDim.x * UNROLL;
+      for (size_t i0 = (size_t)blockIdx.x * blockDim.x * UNROLL + tid; i0 < nvec; i0 += step) {
+        Pack<T> v[UNROLL];
 #pragma unroll
-      for (int u = 0; u < UNROLL; ++u) {
-        const size_t i = i0 + (size_t)u * blockDim.x;
-        if (i < nvec) v[u] = Multimem<T, Op>::ld_reduce(src + i * 16);
-      }
+        for (int u = 0; u < UNROLL; ++u) {
+          const size_t i = i0 + (size_t)u * blockDim.x;
+          if (i < nvec) v[u] = Multimem<T, Op>::ld_reduce(src + i * 16);
+        }
 #pragma unroll
-      for (int u = 0; u < UNROLL; ++u) {
-        const size_t i = i0 + (size_t)u * blockDim.x;
-        if (i < nvec) st_pack<T>(out + i * 16, v[u]);
+        for (int u = 0; u < UNROLL; ++u) {
+          const size_t i = i0 + (size_t)u * blockDim.x;
+          if (i < nvec) st_pack<T>(out + i * 16, v[u]);
+        }
       }
+    } else { // P2P, scalar, rank order (every rank takes this branch: the decision uses exchanged offsets only)
+      for (size_t e = (size_t)blockIdx.x * blockDim.x + tid; e < count; e += (size_t)gridDim.x * blockDim.x)
+        reinterpret_cast<T*>(out)[e] = reduce_ranks<T, Op>([&](int r) { return c.base[r] + s_a[r] + (size_t)c.rank * blk_bytes; }, n, e);
     }
-  } else { // P2P, scalar, rank order (every rank takes this branch: the decision uses exchanged offsets only)
-    for (size_t e = (size_t)blockIdx.x * blockDim.x + tid; e < count; e += (size_t)gridDim.x * blockDim.x) {
-      T acc = reinterpret_cast<const volatile T*>(c.base[0] + s_a[0] + (size_t)c.rank * blk_bytes)[e];
-      for (int r = 1; r < n; ++r) acc = Op::template apply<T>(acc, reinterpret_cast<const volatile T*>(c.base[r] + s_a[r] + (size_t)c.rank * blk_bytes)[e]);
-      reinterpret_cast<T*>(out)[e] = acc;
-    }
-  }
-  sync_end(c);
+  });
 }
 
 // Coherent (system-scope) loads of one access unit, for data that a peer rewrites during the
@@ -1266,10 +1261,20 @@ __device__ __forceinline__ bool all_aligned_to(const uint64_t* s_a, const uint64
   return (m & (unit - 1)) == 0;
 }
 
+// Runs body(unit, unroll) with the host's unit U and UNROLL when every rank's offsets allow U
+// (`aligned`, typically all_aligned_to), else with bytes and an unroll of 1.  `unit` is a value of
+// the unit type and `unroll` a std::integral_constant, so the body names them as decltype(unit)
+// and unroll.
+template <typename U, int UNROLL, typename Body>
+__device__ __forceinline__ void unit_or_bytes(bool aligned, Body body) {
+  if (sizeof(U) == 1 || aligned) body(U{}, std::integral_constant<int, UNROLL>{});
+  else body((unsigned char)0, std::integral_constant<int, 1>{});
+}
+
 // The copy loop of the push and pull bodies: units [lo, hi) of src, grid-strided, UNROLL loads in
-// flight per thread, then each unit stored to the first `ntargets` of dst[0..MAXT).  push_rotated
-// keeps its own single-target loop: inside its loop over targets, this one compiled to more
-// registers.
+// flight per thread, then each unit stored to the first `ntargets` of dst[0..MAXT).  Written out
+// rather than built on `unrolled`, which changed the SASS of allgather_push_kernel and
+// bcast_nvls_kernel.
 template <typename U, int UNROLL, int MAXT>
 __device__ __forceinline__ void copy_units(const U* src, U* const* dst, int ntargets, size_t lo, size_t hi) {
   const size_t step = (size_t)gridDim.x * blockDim.x * UNROLL;
@@ -1334,15 +1339,11 @@ __device__ __forceinline__ void allgather_push_body(const Comm& c, const uint64_
 template <typename U, int UNROLL>
 __global__ void __launch_bounds__(kThreads, 1)
 allgather_push_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t bytes_per_rank) {
-  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
-  const bool call_ok = sync_start(c, send_off, recv_off, s_a, s_b);
-  if (!call_ok) { // ranks disagree about this call: touch nothing, leave through the end barrier
-    sync_end_failed(c);
-    return;
-  }
-  if (sizeof(U) == 1 || all_aligned_to(s_a, s_b, c.n, sizeof(U))) push_block_body<U, UNROLL>(c, s_a, s_b, (uint64_t)c.rank * bytes_per_rank, bytes_per_rank, -1);
-  else push_block_body<unsigned char, 1>(c, s_a, s_b, (uint64_t)c.rank * bytes_per_rank, bytes_per_rank, -1);
-  sync_end(c);
+  collective(c, send_off, recv_off, [&](const uint64_t* s_a, const uint64_t* s_b) {
+    unit_or_bytes<U, UNROLL>(all_aligned_to(s_a, s_b, c.n, sizeof(U)), [&](auto unit, auto unroll) {
+      push_block_body<decltype(unit), unroll>(c, s_a, s_b, (uint64_t)c.rank * bytes_per_rank, bytes_per_rank, -1);
+    });
+  });
 }
 
 // Ring allgather: step s pulls block (r - s - 1) from the predecessor.
@@ -1379,15 +1380,11 @@ __device__ __forceinline__ void allgather_ring_body(const Comm& c, const uint64_
 template <typename U>
 __global__ void __launch_bounds__(kThreads, 1)
 allgather_ring_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t bytes_per_rank) {
-  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
-  const bool call_ok = sync_start(c, send_off, recv_off, s_a, s_b);
-  if (!call_ok) { // ranks disagree about this call: touch nothing, leave through the end barrier
-    sync_end_failed(c);
-    return;
-  }
-  if (sizeof(U) == 1 || all_aligned_to(s_a, s_b, c.n, sizeof(U))) allgather_ring_body<U>(c, s_a, s_b, bytes_per_rank);
-  else allgather_ring_body<unsigned char>(c, s_a, s_b, bytes_per_rank);
-  sync_end(c);
+  collective(c, send_off, recv_off, [&](const uint64_t* s_a, const uint64_t* s_b) {
+    unit_or_bytes<U, 1>(all_aligned_to(s_a, s_b, c.n, sizeof(U)), [&](auto unit, auto) {
+      allgather_ring_body<decltype(unit)>(c, s_a, s_b, bytes_per_rank);
+    });
+  });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1429,56 +1426,35 @@ __device__ __forceinline__ void bcast_body(const Comm& c, const uint64_t* s_a, s
 template <typename U, int UNROLL>
 __global__ void __launch_bounds__(kThreads, 1)
 bcast_kernel(Comm c, uint64_t buf_off, size_t bytes, int root, int mode) {
-  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
-  const bool call_ok = sync_start(c, buf_off, buf_off, s_a, s_b);
-  if (!call_ok) { // ranks disagree about this call: touch nothing, leave through the end barrier
-    sync_end_failed(c);
-    return;
-  }
-  if (sizeof(U) == 1 || all_aligned_to(s_a, s_b, c.n, sizeof(U))) bcast_body<U, UNROLL>(c, s_a, bytes, root, mode);
-  else bcast_body<unsigned char, 1>(c, s_a, bytes, root, mode);
-  sync_end(c);
+  collective(c, buf_off, buf_off, [&](const uint64_t* s_a, const uint64_t* s_b) {
+    unit_or_bytes<U, UNROLL>(all_aligned_to(s_a, s_b, c.n, sizeof(U)), [&](auto unit, auto unroll) {
+      bcast_body<decltype(unit), unroll>(c, s_a, bytes, root, mode);
+    });
+  });
 }
 
 // Bcast through the switch: root streams its buffer once into the multicast address.
 template <int UNROLL>
 __global__ void __launch_bounds__(kThreads, 1)
 bcast_nvls_kernel(Comm c, uint64_t buf_off, size_t bytes, int root) {
-  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
-  const bool call_ok = sync_start(c, buf_off, buf_off, s_a, s_b);
-  if (!call_ok) { // ranks disagree about this call: touch nothing, leave through the end barrier
-    sync_end_failed(c);
-    return;
-  }
-  const int n = c.n;
-  bool symmetric = (buf_off & 15) == 0 && (bytes & 15) == 0;
-  for (int r = 0; r < n; ++r) symmetric = symmetric && s_a[r] == buf_off;
-  if (symmetric) {
-    if (c.rank == root) {
-      const size_t nvec = bytes / 16;
-      const char* src = c.base[root] + buf_off;
-      char* dst = c.mc + buf_off;
-      const size_t step = (size_t)gridDim.x * blockDim.x * UNROLL;
-      for (size_t i0 = (size_t)blockIdx.x * blockDim.x * UNROLL + threadIdx.x; i0 < nvec; i0 += step) {
-        uint4 v[UNROLL];
-#pragma unroll
-        for (int u = 0; u < UNROLL; ++u) {
-          const size_t i = i0 + (size_t)u * blockDim.x;
-          if (i < nvec) v[u] = ldg16(src + i * 16);
-        }
-#pragma unroll
-        for (int u = 0; u < UNROLL; ++u) {
-          const size_t i = i0 + (size_t)u * blockDim.x;
-          if (i < nvec) multimem_st16(dst + i * 16, v[u]);
-        }
+  collective(c, buf_off, buf_off, [&](const uint64_t* s_a, const uint64_t* s_b) {
+    const int n = c.n;
+    bool symmetric = (buf_off & 15) == 0 && (bytes & 15) == 0;
+    for (int r = 0; r < n; ++r) symmetric = symmetric && s_a[r] == buf_off;
+    if (symmetric) {
+      if (c.rank == root) {
+        const char* src = c.base[root] + buf_off;
+        char* dst = c.mc + buf_off;
+        unrolled<UNROLL, uint4>(
+            0, bytes / 16, [&](size_t i, uint4& v) { v = ldg16(src + i * 16); },
+            [&](size_t i, const uint4& v) { multimem_st16(dst + i * 16, v); });
       }
+    } else { // different heap offsets per rank: pull from root
+      unit_or_bytes<uint4, UNROLL>((bytes & 15) == 0 && all_aligned_to(s_a, s_b, n, 16), [&](auto unit, auto unroll) {
+        bcast_body<decltype(unit), unroll>(c, s_a, bytes, root, 0);
+      });
     }
-  } else if ((bytes & 15) == 0 && all_aligned_to(s_a, s_b, n, 16)) { // different heap offsets per rank: pull from root
-    bcast_body<uint4, UNROLL>(c, s_a, bytes, root, 0);
-  } else {
-    bcast_body<unsigned char, 1>(c, s_a, bytes, root, 0);
-  }
-  sync_end(c);
+  });
 }
 
 // Bcast, scatter + multicast: the buffer is cut into ownership blocks (Owner, as in the allreduce);
@@ -1490,41 +1466,22 @@ bcast_nvls_kernel(Comm c, uint64_t buf_off, size_t bytes, int root) {
 template <int UNROLL>
 __global__ void __launch_bounds__(kThreads, 1)
 bcast_nvls2_kernel(Comm c, uint64_t buf_off, size_t bytes, int root, uint32_t shift) {
-  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
-  const bool call_ok = sync_start(c, buf_off, buf_off, s_a, s_b);
-  if (!call_ok) {
-    sync_end_failed(c);
-    return;
-  }
-  const int n = c.n;
-  bool symmetric = (buf_off & 15) == 0 && (bytes & 15) == 0;
-  for (int r = 0; r < n; ++r) symmetric = symmetric && s_a[r] == buf_off;
-  if (symmetric) {
-    const size_t nvec = bytes / 16;
-    const Owner own(nvec, shift, n, c.rank);
-    const char* src = c.base[root] + buf_off;
-    char* dst = c.mc + buf_off;
-    const size_t tid = threadIdx.x;
-    const size_t step = (size_t)gridDim.x * blockDim.x * UNROLL;
-    for (size_t l0 = (size_t)blockIdx.x * blockDim.x * UNROLL + tid; l0 < own.slots; l0 += step) {
-      uint4 v[UNROLL];
-      size_t gi[UNROLL];
-#pragma unroll
-      for (int u = 0; u < UNROLL; ++u) {
-        const size_t l = l0 + (size_t)u * blockDim.x;
-        gi[u] = l < own.slots ? own.global(l) : nvec;
-        if (gi[u] < nvec) v[u] = ldg16(src + gi[u] * 16);
-      }
-#pragma unroll
-      for (int u = 0; u < UNROLL; ++u)
-        if (gi[u] < nvec) multimem_st16(dst + gi[u] * 16, v[u]);
+  collective(c, buf_off, buf_off, [&](const uint64_t* s_a, const uint64_t* s_b) {
+    const int n = c.n;
+    bool symmetric = (buf_off & 15) == 0 && (bytes & 15) == 0;
+    for (int r = 0; r < n; ++r) symmetric = symmetric && s_a[r] == buf_off;
+    if (symmetric) {
+      const Owner own(bytes / 16, shift, n, c.rank);
+      const char* src = c.base[root] + buf_off;
+      char* dst = c.mc + buf_off;
+      unrolled_owned<UNROLL, uint4>(
+          own, blockIdx.x, gridDim.x, [&](size_t g, uint4& v) { v = ldg16(src + g * 16); }, [&](size_t g, const uint4& v) { multimem_st16(dst + g * 16, v); });
+    } else { // different heap offsets per rank: fused P2P two-shot
+      unit_or_bytes<uint4, UNROLL>((bytes & 15) == 0 && all_aligned_to(s_a, s_b, n, 16), [&](auto unit, auto unroll) {
+        bcast_body<decltype(unit), unroll>(c, s_a, bytes, root, 1);
+      });
     }
-  } else if ((bytes & 15) == 0 && all_aligned_to(s_a, s_b, n, 16)) { // different heap offsets per rank: fused P2P two-shot
-    bcast_body<uint4, UNROLL>(c, s_a, bytes, root, 1);
-  } else {
-    bcast_body<unsigned char, 1>(c, s_a, bytes, root, 1);
-  }
-  sync_end(c);
+  });
 }
 
 // Allgather through the switch: every rank streams its block once from local HBM into the
@@ -1532,39 +1489,21 @@ bcast_nvls2_kernel(Comm c, uint64_t buf_off, size_t bytes, int root, uint32_t sh
 template <int UNROLL>
 __global__ void __launch_bounds__(kThreads, 1)
 allgather_nvls_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t bytes_per_rank) {
-  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
-  const bool call_ok = sync_start(c, send_off, recv_off, s_a, s_b);
-  if (!call_ok) {
-    sync_end_failed(c);
-    return;
-  }
-  const int n = c.n;
-  bool symmetric = ((recv_off | bytes_per_rank) & 15) == 0;
-  for (int r = 0; r < n; ++r) symmetric = symmetric && s_b[r] == recv_off && (s_a[r] & 15) == 0;
-  if (symmetric) {
-    const size_t nvec = bytes_per_rank / 16;
-    const char* src = c.base[c.rank] + send_off;
-    char* dst = c.mc + recv_off + (size_t)c.rank * bytes_per_rank;
-    const size_t step = (size_t)gridDim.x * blockDim.x * UNROLL;
-    for (size_t i0 = (size_t)blockIdx.x * blockDim.x * UNROLL + threadIdx.x; i0 < nvec; i0 += step) {
-      uint4 v[UNROLL];
-#pragma unroll
-      for (int u = 0; u < UNROLL; ++u) {
-        const size_t i = i0 + (size_t)u * blockDim.x;
-        if (i < nvec) v[u] = ldg16(src + i * 16);
-      }
-#pragma unroll
-      for (int u = 0; u < UNROLL; ++u) {
-        const size_t i = i0 + (size_t)u * blockDim.x;
-        if (i < nvec) multimem_st16(dst + i * 16, v[u]);
-      }
+  collective(c, send_off, recv_off, [&](const uint64_t* s_a, const uint64_t* s_b) {
+    const int n = c.n;
+    bool symmetric = ((recv_off | bytes_per_rank) & 15) == 0;
+    for (int r = 0; r < n; ++r) symmetric = symmetric && s_b[r] == recv_off && (s_a[r] & 15) == 0;
+    if (symmetric) {
+      const char* src = c.base[c.rank] + send_off;
+      char* dst = c.mc + recv_off + (size_t)c.rank * bytes_per_rank;
+      unrolled<UNROLL, uint4>(
+          0, bytes_per_rank / 16, [&](size_t i, uint4& v) { v = ldg16(src + i * 16); }, [&](size_t i, const uint4& v) { multimem_st16(dst + i * 16, v); });
+    } else { // different heap offsets per rank: P2P push
+      unit_or_bytes<uint4, UNROLL>((bytes_per_rank & 15) == 0 && all_aligned_to(s_a, s_b, n, 16), [&](auto unit, auto unroll) {
+        allgather_push_body<decltype(unit), unroll>(c, s_a, s_b, bytes_per_rank);
+      });
     }
-  } else if ((bytes_per_rank & 15) == 0 && all_aligned_to(s_a, s_b, n, 16)) { // different heap offsets per rank: P2P push
-    allgather_push_body<uint4, UNROLL>(c, s_a, s_b, bytes_per_rank);
-  } else {
-    allgather_push_body<unsigned char, 1>(c, s_a, s_b, bytes_per_rank);
-  }
-  sync_end(c);
+  });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1572,7 +1511,9 @@ allgather_nvls_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t bytes
 // push, n write streams per GPU, targets rotated so that the ranks do not all hit one peer.
 // ---------------------------------------------------------------------------------------------
 // Block j of this rank's send, len(j) bytes at src(j), goes to dst(j) in rank j's heap; targets
-// rotated with the own block last (a local copy).  Each block is grid-strided over all CTAs.
+// rotated with the own block last (a local copy).  Each block is grid-strided over all CTAs.  The
+// loop is written out: through copy_units or `unrolled`, inside this loop over targets, the
+// kernels compiled to more registers.
 template <typename U, int UNROLL, typename Src, typename Dst, typename Len>
 __device__ __forceinline__ void push_rotated(const Comm& c, Src src, Dst dst, Len len) {
   const int n = c.n;
@@ -1608,15 +1549,11 @@ __device__ __forceinline__ void alltoall_body(const Comm& c, const uint64_t* s_a
 template <typename U, int UNROLL>
 __global__ void __launch_bounds__(kThreads, 1)
 alltoall_kernel(Comm c, uint64_t send_off, uint64_t recv_off, size_t bytes_per_block) {
-  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
-  const bool call_ok = sync_start(c, send_off, recv_off, s_a, s_b);
-  if (!call_ok) {
-    sync_end_failed(c);
-    return;
-  }
-  if (sizeof(U) == 1 || all_aligned_to(s_a, s_b, c.n, sizeof(U))) alltoall_body<U, UNROLL>(c, s_a, s_b, bytes_per_block);
-  else alltoall_body<unsigned char, 1>(c, s_a, s_b, bytes_per_block);
-  sync_end(c);
+  collective(c, send_off, recv_off, [&](const uint64_t* s_a, const uint64_t* s_b) {
+    unit_or_bytes<U, UNROLL>(all_aligned_to(s_a, s_b, c.n, sizeof(U)), [&](auto unit, auto unroll) {
+      alltoall_body<decltype(unit), unroll>(c, s_a, s_b, bytes_per_block);
+    });
+  });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1647,15 +1584,11 @@ __device__ __forceinline__ void gatherv_push_body(const Comm& c, const uint64_t*
 template <typename U, int UNROLL>
 __global__ void __launch_bounds__(kThreads, 1)
 gatherv_push_kernel(Comm c, uint64_t send_off, uint64_t recv_off, VTable vt, int only_dst) {
-  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
-  const bool call_ok = sync_start(c, send_off, recv_off, s_a, s_b);
-  if (!call_ok) {
-    sync_end_failed(c);
-    return;
-  }
-  if (sizeof(U) == 1 || all_aligned_to(s_a, s_b, c.n, sizeof(U))) gatherv_push_body<U, UNROLL>(c, s_a, s_b, vt, only_dst);
-  else gatherv_push_body<unsigned char, 1>(c, s_a, s_b, vt, only_dst);
-  sync_end(c);
+  collective(c, send_off, recv_off, [&](const uint64_t* s_a, const uint64_t* s_b) {
+    unit_or_bytes<U, UNROLL>(all_aligned_to(s_a, s_b, c.n, sizeof(U)), [&](auto unit, auto unroll) {
+      gatherv_push_body<decltype(unit), unroll>(c, s_a, s_b, vt, only_dst);
+    });
+  });
 }
 
 // Every rank pulls its block [off[rank], off[rank+1]) of root's send through the peer mapping into
@@ -1675,15 +1608,11 @@ __device__ __forceinline__ void scatterv_pull_body(const Comm& c, const uint64_t
 template <typename U, int UNROLL>
 __global__ void __launch_bounds__(kThreads, 1)
 scatterv_pull_kernel(Comm c, uint64_t send_off, uint64_t recv_off, VTable vt, int root) {
-  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
-  const bool call_ok = sync_start(c, send_off, recv_off, s_a, s_b);
-  if (!call_ok) {
-    sync_end_failed(c);
-    return;
-  }
-  if (sizeof(U) == 1 || all_aligned_to(s_a, s_b, c.n, sizeof(U))) scatterv_pull_body<U, UNROLL>(c, s_a, s_b, vt, root);
-  else scatterv_pull_body<unsigned char, 1>(c, s_a, s_b, vt, root);
-  sync_end(c);
+  collective(c, send_off, recv_off, [&](const uint64_t* s_a, const uint64_t* s_b) {
+    unit_or_bytes<U, UNROLL>(all_aligned_to(s_a, s_b, c.n, sizeof(U)), [&](auto unit, auto unroll) {
+      scatterv_pull_body<decltype(unit), unroll>(c, s_a, s_b, vt, root);
+    });
+  });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1713,14 +1642,9 @@ __host__ __device__ __forceinline__ Split16 split16(uint64_t addr, size_t count,
   return {head, nvec, count - head - nvec * epv};
 }
 
-// Element e of this rank's block, reduced over the n sources in rank order.
-template <typename T, typename Op>
-__device__ __forceinline__ T rsv_element(const char* const* src, int n, size_t e) {
-  T acc = reinterpret_cast<const volatile T*>(src[0])[e];
-  for (int r = 1; r < n; ++r) acc = Op::template apply<T>(acc, reinterpret_cast<const volatile T*>(src[r])[e]);
-  return acc;
-}
-
+// The vector loop loads rank by rank (UNROLL vectors of one rank in flight, then combined), not
+// vector by vector as `unrolled` would.  The start/end barriers are written out: through
+// `collective` this kernel compiled to different SASS.
 template <typename T, typename Op, int UNROLL>
 __global__ void __launch_bounds__(kThreads, 1)
 reduce_scatterv_kernel(Comm c, uint64_t send_off, uint64_t recv_off, VTable vt) {
@@ -1745,7 +1669,7 @@ reduce_scatterv_kernel(Comm c, uint64_t send_off, uint64_t recv_off, VTable vt) 
   const Split16 sp = agree ? split16(send_off + lo, count, sizeof(T)) : Split16{count, 0, 0};
   const size_t tid = threadIdx.x;
   const size_t gtid = (size_t)blockIdx.x * blockDim.x + tid, gstride = (size_t)gridDim.x * blockDim.x;
-  for (size_t e = gtid; e < sp.head; e += gstride) out[e] = rsv_element<T, Op>(src, n, e);
+  for (size_t e = gtid; e < sp.head; e += gstride) out[e] = reduce_ranks<T, Op>([&](int r) { return src[r]; }, n, e);
   const size_t v0 = sp.head * sizeof(T); // byte offset of the first whole vector in every source
   const bool wide_out = (recv_off & 15) == res;
   const size_t step = gstride * UNROLL;
@@ -1779,7 +1703,7 @@ reduce_scatterv_kernel(Comm c, uint64_t send_off, uint64_t recv_off, VTable vt) 
       }
     }
   }
-  for (size_t e = sp.head + sp.nvec * EPV + gtid; e < count; e += gstride) out[e] = rsv_element<T, Op>(src, n, e);
+  for (size_t e = sp.head + sp.nvec * EPV + gtid; e < count; e += gstride) out[e] = reduce_ranks<T, Op>([&](int r) { return src[r]; }, n, e);
   sync_end(c);
 }
 
@@ -1850,8 +1774,9 @@ alltoallv_push_kernel(Comm c, uint64_t send_off, uint64_t recv_off, VTable sv, V
   }
   uint64_t m = 0;
   for (int r = 0; r < c.n; ++r) m |= s_b[r];
-  if (sizeof(U) == 1 || (m & (sizeof(U) - 1)) == 0) alltoallv_push_body<U, UNROLL>(c, s_src, s_a, s_b);
-  else alltoallv_push_body<unsigned char, 1>(c, s_src, s_a, s_b);
+  unit_or_bytes<U, UNROLL>((m & (sizeof(U) - 1)) == 0, [&](auto unit, auto unroll) {
+    alltoallv_push_body<decltype(unit), unroll>(c, s_src, s_a, s_b);
+  });
   sync_end(c);
 }
 
@@ -1872,20 +1797,7 @@ copy_bytes_kernel(unsigned char* __restrict__ dst, const unsigned char* __restri
     const size_t nvec = (bytes - head) / 16;
     const unsigned char* s = src + head;
     unsigned char* d = dst + head;
-    const size_t step = stride * UNROLL;
-    for (size_t i0 = (size_t)blockIdx.x * blockDim.x * UNROLL + threadIdx.x; i0 < nvec; i0 += step) {
-      uint4 v[UNROLL];
-#pragma unroll
-      for (int u = 0; u < UNROLL; ++u) {
-        const size_t i = i0 + (size_t)u * blockDim.x;
-        if (i < nvec) v[u] = ldg16(s + i * 16);
-      }
-#pragma unroll
-      for (int u = 0; u < UNROLL; ++u) {
-        const size_t i = i0 + (size_t)u * blockDim.x;
-        if (i < nvec) stg16(d + i * 16, v[u]);
-      }
-    }
+    unrolled<UNROLL, uint4>(0, nvec, [&](size_t i, uint4& v) { v = ldg16(s + i * 16); }, [&](size_t i, const uint4& v) { stg16(d + i * 16, v); });
     for (size_t i = head + nvec * 16 + tid; i < bytes; i += stride) dst[i] = src[i];
   } else {
     for (size_t i = tid; i < bytes; i += stride) dst[i] = src[i];
@@ -1934,14 +1846,6 @@ copy_local_kernel(unsigned char* __restrict__ dst, const unsigned char* __restri
 __device__ __forceinline__ uint4* ll_lane(const Comm& c, int owner, uint32_t parity, int src) {
   return reinterpret_cast<uint4*>(c.base[owner] + kLLOff) + ((size_t)parity * c.n + src) * ll_cells(c.n);
 }
-__device__ __forceinline__ void st_cell(uint4* p, uint4 v) {
-  asm volatile("st.volatile.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-__device__ __forceinline__ uint4 ld_cell(const uint4* p) {
-  uint4 v;
-  asm volatile("ld.volatile.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
-  return v;
-}
 template <typename T> struct LLCodec; // 8 payload bytes <-> elements
 template <> struct LLCodec<float> {
   static constexpr int EPC = 2;
@@ -1979,7 +1883,7 @@ allreduce_ll_kernel(Comm c, const T* __restrict__ send, T* recv, size_t count, u
     const uint4 cell = make_uint4(w0, seq, w1, seq);
     for (int j = 1; j < n; ++j) { // push to every peer, starting after this rank
       const int r = (c.rank + j) % n;
-      st_cell(ll_lane(c, r, parity, c.rank) + i, cell);
+      st_cell16(ll_lane(c, r, parity, c.rank) + i, cell);
     }
   }
   // phase 2: reduce the own lanes in rank order.  The n-1 cells of one element are loaded together
@@ -1993,9 +1897,10 @@ allreduce_ll_kernel(Comm c, const T* __restrict__ send, T* recv, size_t count, u
 #pragma unroll
     for (int r = 0; r < kMaxRanks; ++r)
       if (r < n && r != c.rank) {
-        got[r] = ld_cell(ll_lane(c, c.rank, parity, r) + i);
+        got[r] = ld_cell16(ll_lane(c, c.rank, parity, r) + i);
         pending |= 1u << r;
       }
+    // the watchdog poll of wait_flag
     unsigned long long t0 = 0;
     uint32_t it = 0;
     for (;;) {
@@ -2007,7 +1912,7 @@ allreduce_ll_kernel(Comm c, const T* __restrict__ send, T* recv, size_t count, u
       if (!pending) break;
 #pragma unroll
       for (int r = 0; r < kMaxRanks; ++r)
-        if ((pending >> r) & 1u) got[r] = ld_cell(ll_lane(c, c.rank, parity, r) + i);
+        if ((pending >> r) & 1u) got[r] = ld_cell16(ll_lane(c, c.rank, parity, r) + i);
       if ((++it & 0xfffu) == 0) {
         const unsigned long long now = globaltimer_ns();
         if (t0 == 0) t0 = now;
@@ -2076,9 +1981,7 @@ __global__ void scrub_kernel(Comm c) {
 
 // A device-wide rendezvous with nothing in between (b200mpi_barrier).
 __global__ void barrier_kernel(Comm c) {
-  __shared__ uint64_t s_a[kMaxRanks], s_b[kMaxRanks];
-  if (sync_start(c, 0, 0, s_a, s_b)) sync_end(c);
-  else sync_end_failed(c);
+  collective(c, 0, 0, [](const uint64_t*, const uint64_t*) {});
 }
 
 } // namespace b200

@@ -1525,121 +1525,126 @@ struct PendingSend { MsgSlot* slot; size_t stage; bool staged; };
 static std::mutex g_pending_mu;
 static std::map<std::pair<int, int>, PendingSend> g_pending; // {dest, tag} -> posted, not yet acknowledged (Isend)
 
+// What Send, Isend and Receive check first, in this order: the data plane, the dtype, the peer, the
+// buffer and the memory kind.  what is "send" or "recv"; es receives the element size.
+static int check_p2p(const char* what, int dtype, int peer, const void* buf, size_t count, int memkind, size_t& es) {
+  int rc = need_data_plane();
+  if (rc) return rc;
+  const bool send = !strcmp(what, "send");
+  auto arg = [&](const std::string& msg) { return fail(B200MPI_ERR_ARG, std::string(what) + ": " + msg); };
+  es = esize(dtype);
+  if (es == 0) return arg("unknown dtype");
+  if (peer < 0 || peer >= g->ctrl.n) return arg((send ? "destination " : "source ") + std::to_string(peer) + " out of range");
+  if (count && !buf) return arg(send ? "NULL buffer with count > 0" : "NULL buffer with capacity > 0");
+  if (memkind != B200MPI_HOST && memkind != B200MPI_DEVICE) return arg("bad memkind");
+  return 0;
+}
+
+// Gives a {peer, tag} taken in `tags` back when the call that took it returns, unless an Isend
+// hands it on to b200mpi_wait (keep).
+struct TagRelease {
+  TagSet& tags;
+  int tag;
+  bool keep = false;
+  ~TagRelease() { if (!keep) tags.remove(tag); }
+};
+
+// The end of a Send, or of an Isend in b200mpi_wait: wait for the receiver's acknowledgement
+// (network.go:569), then free the staging block and the slot.  After a failure (rc != 0, or no
+// acknowledgement within the watchdog time) the post is withdrawn and the failure's message kept.
+static int finish_send(const char* what, const PendingSend& ps, int rc) {
+  if (rc == 0) {
+    Spinner sp(g->watchdog_ns);
+    while (ps.slot->state.load(std::memory_order_acquire) != kDone)
+      if (!sp.step()) { rc = fail(B200MPI_ERR_TIMEOUT, std::string(what) + ": no matching receive within the watchdog time"); break; }
+  }
+  if (rc == 0) {
+    if (ps.staged) g->heap.free_off(ps.stage);
+    ps.slot->state.store(kFree, std::memory_order_release);
+  } else {
+    const std::string why = t_err;
+    if (retire_failed_send(ps.slot) && ps.staged) g->heap.free_off(ps.stage);
+    t_err = why;
+  }
+  return rc;
+}
+
 // wait_ack = true: mpi.Send (network.go:518-572), returns after the receiver's acknowledgement.
 // wait_ack = false: the Send of the design sketched in mpi.go:132-152 -- returns once the data has
 // left the caller's buffer ("sent on connection"); b200mpi_wait collects the acknowledgement.
 static int do_send(const void* buf, size_t count, int dtype, int dest, int tag, int memkind, bool wait_ack) {
-  int rc = need_data_plane();
+  size_t es;
+  int rc = check_p2p("send", dtype, dest, buf, count, memkind, es);
   if (rc) return rc;
-  const size_t es = esize(dtype);
-  if (es == 0) return fail(B200MPI_ERR_ARG, "send: unknown dtype");
-  if (dest < 0 || dest >= g->ctrl.n) return fail(B200MPI_ERR_ARG, "send: destination " + std::to_string(dest) + " out of range");
-  if (count && !buf) return fail(B200MPI_ERR_ARG, "send: NULL buffer with count > 0");
-  if (memkind != B200MPI_HOST && memkind != B200MPI_DEVICE) return fail(B200MPI_ERR_ARG, "send: bad memkind");
   if (!g->sendtags[dest].add(tag)) return fail(B200MPI_ERR_TAG_EXISTS, "Tag " + std::to_string(tag) + " already in use sending"); // mpi.go:180-182
-  const size_t bytes = count * es;
-  const int me = g->ctrl.rank;
+  TagRelease held{g->sendtags[dest], tag};
   MsgSlot* slot = claim_slot(dest);
-  if (!slot) {
-    g->sendtags[dest].remove(tag);
-    return fail(B200MPI_ERR_TIMEOUT, "send: no free mailbox slot");
-  }
-  slot->tag = tag;
-  slot->dtype = (uint32_t)dtype;
-  slot->result = 0;
-  slot->count = count;
-  slot->total_bytes = bytes;
-  slot->done.store(0, std::memory_order_relaxed);
+  if (!slot) return fail(B200MPI_ERR_TIMEOUT, "send: no free mailbox slot");
+  const size_t bytes = count * es;
+  // The layout.  Direct: the receiver pulls straight out of the caller's heap buffer (a Send only;
+  // an Isend leaves the caller's buffer free).  Staged whole: an Isend keeps the whole message in the
+  // staging block until Wait, and a small host slice goes through a mapped pinned bounce, where one
+  // kernel moves it into the heap (the SMs read host memory over PCIe).  Otherwise a Send streams the
+  // message through a ring of up to kMsgRegions chunks.
+  PendingSend ps{slot, 0, false};
   size_t off = 0;
-  size_t stage = 0;
-  bool staged = false;
-  cudaStream_t s = nullptr;
-  Ctx::P2PBounce* bounce = nullptr;
-  rc = 0;
-  if (bytes == 0 || (wait_ack && memkind == B200MPI_DEVICE && g->heap.contains(buf, bytes, off))) {
-    // heap-resident: the receiver pulls straight out of the caller's buffer
-    slot->chunk_bytes = bytes;
-    slot->nregions = 1;
-    slot->region_off[0] = off;
-    slot->posted.store(bytes, std::memory_order_relaxed);
-    slot->state.store(kPosted, std::memory_order_release);
-  } else if (memkind == B200MPI_HOST && g->p2p_fast && bytes <= Ctx::kP2PBounceBytes && (bounce = acquire_bounce()) != nullptr) {
-    // small host slice: memcpy into a mapped pinned buffer, one kernel moves it into the heap (the
-    // SMs read host memory over PCIe), the host spins on the completion word, then the whole
-    // message is posted at once
-    staged = true;
-    if (g->heap.alloc(bytes, stage)) {
-      release_bounce(bounce);
-      slot->state.store(kFree, std::memory_order_release);
-      g->sendtags[dest].remove(tag);
-      return fail(B200MPI_ERR_NOMEM, "send: symmetric heap exhausted while staging (raise B200MPI_HEAP_BYTES)");
-    }
-    memcpy(bounce->host, buf, bytes);
-    s = borrow_stream();
-    rc = copy_and_wait(bounce, (char*)g->heap.base[me] + stage, bounce->dev, bytes, s);
-    release_bounce(bounce);
-    slot->chunk_bytes = bytes;
-    slot->nregions = 1;
-    slot->region_off[0] = stage;
-    slot->posted.store(rc == 0 ? bytes : 0, std::memory_order_relaxed);
-    slot->state.store(kPosted, std::memory_order_release);
-  } else {
-    staged = true;
-    // Isend keeps the whole message in the staging block until Wait; Send streams it through a ring
-    const size_t chunk = wait_ack ? std::min(bytes, p2p_chunk(bytes, memkind)) : bytes;
-    const size_t nchunks = (bytes + chunk - 1) / chunk;
-    const size_t nreg = std::min<size_t>(nchunks, kMsgRegions);
-    if (g->heap.alloc(chunk * nreg, stage)) {
-      slot->state.store(kFree, std::memory_order_release);
-      g->sendtags[dest].remove(tag);
-      return fail(B200MPI_ERR_NOMEM, "send: symmetric heap exhausted while staging (raise B200MPI_HEAP_BYTES)");
-    }
+  const bool direct = bytes == 0 || (wait_ack && memkind == B200MPI_DEVICE && g->heap.contains(buf, bytes, off));
+  Ctx::P2PBounce* bounce = !direct && memkind == B200MPI_HOST && g->p2p_fast && bytes <= Ctx::kP2PBounceBytes ? acquire_bounce() : nullptr;
+  const size_t chunk = direct || bounce || !wait_ack ? bytes : std::min(bytes, p2p_chunk(bytes, memkind));
+  const size_t nchunks = direct ? 0 : (bytes + chunk - 1) / chunk;
+  const size_t nreg = std::min<size_t>(std::max<size_t>(nchunks, 1), kMsgRegions);
+  if (!direct) {
+    if (g->heap.alloc(chunk * nreg, ps.stage)) rc = fail(B200MPI_ERR_NOMEM, "send: symmetric heap exhausted while staging (raise B200MPI_HEAP_BYTES)");
+    else ps.staged = true;
+  }
+  if (rc == 0) {
+    slot->tag = tag;
+    slot->dtype = (uint32_t)dtype;
+    slot->result = 0;
+    slot->count = count;
+    slot->total_bytes = bytes;
     slot->chunk_bytes = chunk;
     slot->nregions = (uint32_t)nreg;
-    for (size_t r = 0; r < nreg; ++r) slot->region_off[r] = stage + r * chunk;
-    slot->posted.store(0, std::memory_order_relaxed);
+    for (size_t r = 0; r < nreg; ++r) slot->region_off[r] = direct ? off : ps.stage + r * chunk;
+    slot->done.store(0, std::memory_order_relaxed);
+    slot->posted.store(direct ? bytes : 0, std::memory_order_relaxed);
     slot->state.store(kPosted, std::memory_order_release);
-    s = borrow_stream();
-    char* base = (char*)g->heap.base[me];
-    for (size_t k = 0; k < nchunks && rc == 0; ++k) {
-      if (k >= nreg) { // the region was used by chunk k-nreg: wait until the receiver drained it
-        Spinner sp(g->watchdog_ns);
-        while (slot->done.load(std::memory_order_acquire) < (k - nreg + 1) * chunk && slot->state.load(std::memory_order_acquire) != kDone)
-          if (!sp.step()) { rc = fail(B200MPI_ERR_TIMEOUT, "send: receiver stalled"); break; }
-        if (rc) break;
-      }
-      if (slot->state.load(std::memory_order_acquire) == kDone) break; // receiver gave up (truncate)
-      const size_t lo = k * chunk, len = std::min(chunk, bytes - lo);
-      cudaError_t e;
-      if (memkind == B200MPI_HOST) e = cudaMemcpyAsync(base + slot->region_off[k % nreg], (const char*)buf + lo, len, cudaMemcpyHostToDevice, s);
-      else { e = cudaSuccess; rc = launch_copy(base + slot->region_off[k % nreg], (const char*)buf + lo, len, s); }
-      if (e == cudaSuccess && rc == 0) e = cudaStreamSynchronize(s);
-      if (e != cudaSuccess) { rc = fail(B200MPI_ERR_CUDA, std::string("send staging: ") + cudaGetErrorString(e)); break; }
-      slot->posted.store(lo + len, std::memory_order_release);
-    }
   }
+  // The fill: each chunk moves into its region and is then published in `posted`.
+  cudaStream_t s = rc == 0 && nchunks ? borrow_stream() : nullptr;
+  char* base = (char*)g->heap.base[g->ctrl.rank];
+  for (size_t k = 0; k < nchunks && rc == 0; ++k) {
+    if (k >= nreg) { // the region was used by chunk k-nreg: wait until the receiver drained it
+      Spinner sp(g->watchdog_ns);
+      while (slot->done.load(std::memory_order_acquire) < (k - nreg + 1) * chunk && slot->state.load(std::memory_order_acquire) != kDone)
+        if (!sp.step()) { rc = fail(B200MPI_ERR_TIMEOUT, "send: receiver stalled"); break; }
+      if (rc) break;
+    }
+    if (slot->state.load(std::memory_order_acquire) == kDone) break; // the receiver gave up (dtype mismatch or failure)
+    const size_t lo = k * chunk, len = std::min(chunk, bytes - lo);
+    char* to = base + slot->region_off[k % nreg];
+    const char* from = (const char*)buf + lo;
+    if (bounce) {
+      memcpy(bounce->host, from, len);
+      rc = copy_and_wait(bounce, to, bounce->dev, len, s);
+    } else {
+      cudaError_t e = cudaSuccess;
+      if (memkind == B200MPI_HOST) e = cudaMemcpyAsync(to, from, len, cudaMemcpyHostToDevice, s);
+      else rc = launch_copy(to, from, len, s);
+      if (e == cudaSuccess && rc == 0) e = cudaStreamSynchronize(s);
+      if (e != cudaSuccess) rc = fail(B200MPI_ERR_CUDA, std::string("send staging: ") + cudaGetErrorString(e));
+    }
+    if (rc == 0) slot->posted.store(lo + len, std::memory_order_release);
+  }
+  if (bounce) release_bounce(bounce);
   if (s) return_stream(s);
   if (rc == 0 && !wait_ack) { // Isend: the acknowledgement is collected by b200mpi_wait
     std::lock_guard<std::mutex> l(g_pending_mu);
-    g_pending[{dest, tag}] = {slot, stage, staged};
+    g_pending[{dest, tag}] = ps;
+    held.keep = true;
     return 0;
   }
-  // wait for the receiver's acknowledgement (network.go:569)
-  if (rc == 0) {
-    Spinner sp(g->watchdog_ns);
-    while (slot->state.load(std::memory_order_acquire) != kDone)
-      if (!sp.step()) { rc = fail(B200MPI_ERR_TIMEOUT, "send: no matching receive within the watchdog time"); break; }
-  }
-  if (rc == 0) {
-    if (staged) g->heap.free_off(stage);
-    slot->state.store(kFree, std::memory_order_release);
-  } else {
-    const std::string why = t_err;
-    if (retire_failed_send(slot) && staged) g->heap.free_off(stage);
-    t_err = why;
-  }
-  g->sendtags[dest].remove(tag);
-  return rc;
+  return finish_send("send", ps, rc);
 }
 
 // mpi.go:146-152 (commented design): block until `destination` confirmed the message sent with
@@ -1655,30 +1660,16 @@ static int do_wait(int dest, int tag) {
     ps = it->second;
     g_pending.erase(it);
   }
-  Spinner sp(g->watchdog_ns);
-  while (ps.slot->state.load(std::memory_order_acquire) != kDone)
-    if (!sp.step()) { rc = fail(B200MPI_ERR_TIMEOUT, "wait: no matching receive within the watchdog time"); break; }
-  if (rc == 0) {
-    if (ps.staged) g->heap.free_off(ps.stage);
-    ps.slot->state.store(kFree, std::memory_order_release);
-  } else {
-    const std::string why = t_err;
-    if (retire_failed_send(ps.slot) && ps.staged) g->heap.free_off(ps.stage);
-    t_err = why;
-  }
-  g->sendtags[dest].remove(tag);
-  return rc;
+  TagRelease held{g->sendtags[dest], tag};
+  return finish_send("wait", ps, 0);
 }
 
 static int do_recv(void* buf, size_t capacity, size_t* count_out, int dtype, int src, int tag, int memkind) {
-  int rc = need_data_plane();
+  size_t es;
+  int rc = check_p2p("recv", dtype, src, buf, capacity, memkind, es);
   if (rc) return rc;
-  const size_t es = esize(dtype);
-  if (es == 0) return fail(B200MPI_ERR_ARG, "recv: unknown dtype");
-  if (src < 0 || src >= g->ctrl.n) return fail(B200MPI_ERR_ARG, "recv: source " + std::to_string(src) + " out of range");
-  if (capacity && !buf) return fail(B200MPI_ERR_ARG, "recv: NULL buffer with capacity > 0");
-  if (memkind != B200MPI_HOST && memkind != B200MPI_DEVICE) return fail(B200MPI_ERR_ARG, "recv: bad memkind");
   if (!g->recvtags[src].add(tag)) return fail(B200MPI_ERR_TAG_EXISTS, "Tag " + std::to_string(tag) + " already in use receiving");
+  TagRelease held{g->recvtags[src], tag};
   const int me = g->ctrl.rank;
   MsgSlot* slot = nullptr;
   {
@@ -1695,82 +1686,62 @@ static int do_recv(void* buf, size_t capacity, size_t* count_out, int dtype, int
         }
       }
       if (slot) break;
-      if (!sp.step()) {
-        g->recvtags[src].remove(tag);
-        return fail(B200MPI_ERR_TIMEOUT, "recv: no matching send within the watchdog time");
-      }
+      if (!sp.step()) return fail(B200MPI_ERR_TIMEOUT, "recv: no matching send within the watchdog time");
     }
   }
   const size_t count = slot->count, bytes = slot->total_bytes;
   if (count_out) *count_out = count;
-  rc = 0;
   if (slot->dtype != (uint32_t)dtype) {
     rc = fail(B200MPI_ERR_ARG, "recv: sender used dtype " + std::to_string(slot->dtype) + ", receiver asked for " + std::to_string(dtype));
   } else if (count > capacity) {
     // Nothing is consumed: the message stays posted so the caller can retry with a buffer of
     // *count_out elements (what gob's slice resize does for the reference, network.go:597).
     slot->state.store(kPosted, std::memory_order_release);
-    g->recvtags[src].remove(tag);
     return fail(B200MPI_ERR_TRUNCATE, "recv: message has " + std::to_string(count) + " elements, capacity is " + std::to_string(capacity));
   }
-  size_t stage = 0, stage_len = 0;
-  cudaStream_t s = nullptr;
+  // The pull unit.  A small message into a host slice, when every chunk has its own region (so the
+  // message lies contiguous in the sender's heap), is pulled whole once all of it is posted: ONE
+  // kernel moves it over NVLink straight into a mapped pinned bounce (the SMs write host memory),
+  // then a memcpy.  Otherwise each chunk is pulled as soon as it is posted, into a device buffer
+  // directly, or through a staging block and a D2H copy into a host slice.
+  const size_t nreg = slot->nregions ? slot->nregions : 1;
   Ctx::P2PBounce* bounce = nullptr;
-  const bool whole = slot->chunk_bytes * (slot->nregions ? slot->nregions : 1) >= bytes; // every chunk has its own region, contiguous in the sender's heap
-  if (rc == 0 && bytes && memkind == B200MPI_HOST && g->p2p_fast && whole && bytes <= Ctx::kP2PBounceBytes && (bounce = acquire_bounce()) != nullptr) {
-    // small message into a host slice: wait until all of it is posted, ONE kernel pulls it over
-    // NVLink straight into a mapped pinned buffer (the SMs write host memory), spin, memcpy out
-    Spinner sp(g->watchdog_ns);
-    while (slot->posted.load(std::memory_order_acquire) < bytes)
-      if (!sp.step()) { rc = fail(B200MPI_ERR_TIMEOUT, "recv: sender stalled"); break; }
-    if (rc == 0) {
-      s = borrow_stream();
-      rc = copy_and_wait(bounce, bounce->dev, (const char*)g->heap.base[src] + slot->region_off[0], bytes, s);
-      if (rc == 0) memcpy(buf, bounce->host, bytes);
-      slot->done.store(bytes, std::memory_order_release);
-    }
-    release_bounce(bounce);
-  } else if (rc == 0 && bytes) {
-    s = borrow_stream();
-    const size_t chunk = slot->chunk_bytes;
-    const size_t nreg = slot->nregions ? slot->nregions : 1;
-    if (memkind == B200MPI_HOST) {
-      stage_len = std::min(bytes, std::max<size_t>(chunk, 1));
-      if (g->heap.alloc(stage_len, stage)) { rc = fail(B200MPI_ERR_NOMEM, "recv: symmetric heap exhausted while staging"); stage_len = 0; }
-    }
-    const char* peer = (const char*)g->heap.base[src];
-    char* mine = (char*)g->heap.base[me];
-    size_t consumed = 0;
-    while (rc == 0 && consumed < bytes) {
-      size_t posted;
-      Spinner sp(g->watchdog_ns);
-      while ((posted = slot->posted.load(std::memory_order_acquire)) <= consumed)
-        if (!sp.step()) { rc = fail(B200MPI_ERR_TIMEOUT, "recv: sender stalled"); break; }
-      if (rc) break;
-      const size_t k = consumed / chunk;
-      const size_t in_chunk = consumed - k * chunk;
-      size_t len = std::min(posted, (k + 1) * chunk) - consumed;
-      const char* from = peer + slot->region_off[k % nreg] + in_chunk;
-      cudaError_t e = cudaSuccess;
-      if (memkind == B200MPI_DEVICE) {
-        rc = launch_copy((char*)buf + consumed, from, len, s);
-      } else {
-        len = std::min(len, stage_len);
-        rc = launch_copy(mine + stage, from, len, s);
-        if (rc == 0) e = cudaMemcpyAsync((char*)buf + consumed, mine + stage, len, cudaMemcpyDeviceToHost, s);
-      }
-      if (rc == 0 && e == cudaSuccess) e = cudaStreamSynchronize(s);
-      if (rc == 0 && e != cudaSuccess) rc = fail(B200MPI_ERR_CUDA, std::string("recv pull: ") + cudaGetErrorString(e));
-      if (rc) break;
-      consumed += len;
-      slot->done.store(consumed, std::memory_order_release);
-    }
+  if (rc == 0 && bytes && memkind == B200MPI_HOST && g->p2p_fast && slot->chunk_bytes * nreg >= bytes && bytes <= Ctx::kP2PBounceBytes) bounce = acquire_bounce();
+  const size_t unit = bounce ? bytes : slot->chunk_bytes;
+  size_t stage = 0;
+  bool staged = false;
+  if (rc == 0 && bytes && !bounce && memkind == B200MPI_HOST) {
+    if (g->heap.alloc(unit, stage)) rc = fail(B200MPI_ERR_NOMEM, "recv: symmetric heap exhausted while staging");
+    else staged = true;
   }
+  cudaStream_t s = rc == 0 && bytes ? borrow_stream() : nullptr;
+  const char* peer = (const char*)g->heap.base[src];
+  char* mine = (char*)g->heap.base[me];
+  for (size_t lo = 0; rc == 0 && lo < bytes; lo += unit) {
+    // the sender publishes `posted` only at the end of a chunk
+    const size_t len = std::min(unit, bytes - lo);
+    Spinner sp(g->watchdog_ns);
+    while (slot->posted.load(std::memory_order_acquire) < lo + len)
+      if (!sp.step()) { rc = fail(B200MPI_ERR_TIMEOUT, "recv: sender stalled"); break; }
+    if (rc) break;
+    const char* from = peer + slot->region_off[lo / unit % nreg];
+    cudaError_t e = cudaSuccess;
+    if (bounce) {
+      rc = copy_and_wait(bounce, bounce->dev, from, len, s);
+      if (rc == 0) memcpy((char*)buf + lo, bounce->host, len);
+    } else {
+      rc = launch_copy(memkind == B200MPI_DEVICE ? (char*)buf + lo : mine + stage, from, len, s);
+      if (rc == 0 && memkind == B200MPI_HOST) e = cudaMemcpyAsync((char*)buf + lo, mine + stage, len, cudaMemcpyDeviceToHost, s);
+      if (rc == 0 && e == cudaSuccess) e = cudaStreamSynchronize(s);
+    }
+    if (rc == 0 && e != cudaSuccess) rc = fail(B200MPI_ERR_CUDA, std::string("recv pull: ") + cudaGetErrorString(e));
+    if (rc == 0) slot->done.store(lo + len, std::memory_order_release);
+  }
+  if (bounce) release_bounce(bounce);
   if (s) return_stream(s);
-  if (stage_len) g->heap.free_off(stage);
+  if (staged) g->heap.free_off(stage);
   slot->result = rc;
   slot->state.store(kDone, std::memory_order_release); // the ack (network.go:617-621)
-  g->recvtags[src].remove(tag);
   return rc;
 }
 

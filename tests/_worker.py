@@ -609,6 +609,52 @@ def scenario_p2p(a):
             got = mpi.Receive(np.zeros(4097, dtype=dt), rank - 1, 3)
             check_equal(got, O.fill(dt, SEED + 5 + rank - 1, 4097), "typed p2p %s" % np.dtype(dt).name)
         done += 1
+    # a Receive with another dtype fails with ERR_ARG and consumes the message; the Send returns and
+    # the tag is usable again
+    x = O.fill(np.float64, SEED + 6, 5000)
+    if even:
+        mpi.Send(x, rank + 1, 12)
+        mpi.Send(x, rank + 1, 12)
+    else:
+        try:
+            mpi.Receive(np.zeros(5000, dtype=np.int64), rank - 1, 12)
+            raise AssertionError("receive with another dtype succeeded")
+        except mpi.MpiError as e:
+            if e.code != L.ERR_ARG:
+                raise
+        check_equal(mpi.Receive(np.zeros(5000), rank - 1, 12), x, "send/receive after a dtype mismatch")
+    done += 1
+    mpi.Barrier()
+    return {"checked": done}
+
+
+def scenario_p2p_torch(a):
+    """Send/Receive of device memory outside the heap: torch CUDA tensors on both sides."""
+    import torch
+    lib = L.load()
+    rank = mpi.Rank()
+    peer = rank ^ 1
+    torch.cuda.set_device(lib.b200mpi_device())
+    done = 0
+    for count in (1, 4097, (7 << 20) // 16 + 3):  # the last spans several 1 MiB staging chunks
+        x = torch.from_numpy(O.fill(np.float64, SEED + 40 + count, count)).cuda()
+        got = torch.full((count + 8,), -1.0, dtype=torch.float64, device="cuda")
+        torch.cuda.synchronize()
+        n = L.ctypes.c_size_t(0)
+        for sender in (0, 1):
+            if rank % 2 == sender:
+                buf = x if sender == 0 else got
+                rc = lib.b200mpi_send(buf.data_ptr(), count, L.F64, peer, 8, L.DEVICE)
+            else:
+                rc = lib.b200mpi_recv(got.data_ptr(), count + 8, L.ctypes.byref(n), L.F64, peer, 8, L.DEVICE)
+                if rc == 0 and n.value != count:
+                    raise AssertionError("torch recv count %d != %d" % (n.value, count))
+            if rc:
+                raise AssertionError("torch p2p count=%d: %s" % (count, L.last_error()))
+        # rank 0's tensor went to rank 1 and came back: both hold it bit for bit, the tail untouched
+        check_equal(got[:count].cpu().numpy(), x.cpu().numpy(), "torch p2p count=%d" % count)
+        check_equal(got[count:].cpu().numpy(), np.full(8, -1.0), "torch p2p tail count=%d" % count)
+        done += 1
     mpi.Barrier()
     return {"checked": done}
 

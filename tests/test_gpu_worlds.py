@@ -21,11 +21,11 @@ def ngpus():
         return 0
 
 
-def world(n, scenario, *args, timeout=900, env=None):  # generous: the pod's host CPUs are shared, a world of 8 Python ranks can start slowly
+def world(n, scenario, *args, timeout=900, env=None, per_rank_env=None):  # generous: the pod's host CPUs are shared, a world of 8 Python ranks can start slowly
     e = dict(ENV)
     if env:
         e.update(env)
-    res = run_world(n, scenario, args=list(args), timeout=timeout, env=e)
+    res = run_world(n, scenario, args=list(args), timeout=timeout, env=e, per_rank_env=per_rank_env)
     assert_world_ok(res)
     return res
 
@@ -76,10 +76,29 @@ def test_unaligned_and_asymmetric_offsets():
     world(4, "unaligned")
 
 
+def bounce_worlds(per_rank_env=None):
+    # examples/bounce: the reference's size ladder (bounce.go:33) up to 1e7 bytes + the 1 MiB float64
+    # point; with 1 MiB chunks the largest sizes wrap the 4-region staging ring
+    world(2, "p2p", "--sizes", "0,1,10,100,1000,10000,100000,1000000,10000000,1048576", env={"B200MPI_STAGE_CHUNK": str(1 << 20)},
+          per_rank_env=per_rank_env)
+    world(4, "p2p", "--sizes", "0,8,4096,1048576", per_rank_env=per_rank_env)
+
+
 def test_bounce_send_receive():
-    # examples/bounce: the reference's size ladder (bounce.go:33) up to 1e7 bytes + the 1 MiB float64 point
-    world(2, "p2p", "--sizes", "0,1,10,100,1000,10000,100000,1000000,10000000,1048576", env={"B200MPI_STAGE_CHUNK": str(1 << 20)})
-    world(4, "p2p", "--sizes", "0,8,4096,1048576")
+    bounce_worlds()
+
+
+@pytest.mark.parametrize("fast_ranks", ["all", "rank0"])
+def test_bounce_send_receive_mapped_bounce(fast_ranks):
+    """The mapped-bounce path (host slices of at most 4 MiB) is off by default when ranks share a GPU,
+    so it is forced on: on every rank, and on rank 0 only, where a bounce sender meets a ring receiver
+    and a ring sender meets a bounce receiver."""
+    bounce_worlds(lambda r: {"B200MPI_P2P_FAST": "1" if fast_ranks == "all" or r == 0 else "0"})
+
+
+def test_send_receive_device_memory_outside_the_heap():
+    # torch CUDA tensors (memkind DEVICE, not in the heap), over several 1 MiB staging chunks
+    world(2, "p2p_torch", env={"B200MPI_STAGE_CHUNK": str(1 << 20)})
 
 
 @pytest.mark.parametrize("n", [1, 2, 4])
@@ -125,6 +144,7 @@ def test_host_slice_pipeline_pageable_and_pinned(n):
 def test_isend_wait():
     world(2, "isend")
     world(4, "isend")
+    world(2, "isend", env={"B200MPI_P2P_FAST": "1"})  # host Isends of at most 4 MiB go through the mapped bounce
 
 
 def test_send_timeout_withdraws_the_post():

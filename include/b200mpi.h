@@ -135,6 +135,10 @@ int b200mpi_recv(void* buf, size_t capacity, size_t* count_out, int dtype, int s
 
 /* ---- collectives (new API; semantics in SURVEY.md 8(c), oracle/collectives.c) -------------- */
 
+/* Bcast, Allreduce and Allgather of host memory from "pipe_min_bytes" (8 MiB, the whole recv for
+ * Allgather) up run a chunked pipeline: one launch per chunk, where device memory runs one launch.  There
+ * every rank must pass the same memkind.  Pageable, pinned and registered host memory may be mixed
+ * across ranks: in a multi-rank world all of them use the same chunks. */
 int b200mpi_bcast(void* buf, size_t count, int dtype, int root, int memkind);
 /* send == recv means in place. */
 int b200mpi_allreduce(const void* send, void* recv, size_t count, int dtype, int op, int memkind);

@@ -956,14 +956,21 @@ static int allreduce_ll_host(const void* send, void* recv, size_t count, int dty
 // ---------------------------------------------------------------------------------------------
 // Host slices (what an unmodified Go caller passes, bounce.go:120-127): H2D, collective and D2H
 // are pipelined in chunks over three streams so PCIe runs in both directions while the GPUs talk.
-// Every rank derives the same chunking from (count, dtype, n), so the per-chunk collectives line
-// up; the signature of each chunk also carries the total count.
+// Every rank derives the same chunking from (count, dtype, n) and the knobs, whatever memory its own
+// buffer lives in (pipe_chunk_elems), so the per-chunk collectives line up; the signature of each
+// chunk also carries the total count.
 //   pinned (cudaHostAlloc / cudaHostRegister'ed) memory: DMA straight from / to the caller's buffer;
 //   pageable memory (a Go slice, a numpy array): through a ring of pinned bounce chunks filled and
 //   drained by the helper threads of CopyPool while the DMA engines work on the neighbours.
 // ---------------------------------------------------------------------------------------------
-static bool is_pinned(const void* p) {
-  if (!p) return true;
+// True when [p, p + bytes) may be DMA'd in place.  A range this rank registered counts only when one
+// registration holds all of it: a neighbour of a registered buffer can start in the page they share,
+// and a copy that starts there runs past the registration (cudaErrorInvalidValue).
+static bool is_pinned(const void* p, size_t bytes) {
+  if (!p || bytes == 0) return true;
+  const uintptr_t a0 = (uintptr_t)p, a1 = a0 + bytes;
+  for (const auto& e : g->registered)
+    if (a0 < e.first + e.second && e.first < a1) return a0 >= e.first && a1 <= e.first + e.second;
   cudaPointerAttributes a;
   if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { (void)cudaGetLastError(); return false; }
   return a.type == cudaMemoryTypeHost || a.type == cudaMemoryTypeManaged;
@@ -971,7 +978,8 @@ static bool is_pinned(const void* p) {
 
 static bool ensure_registered(const void* p, size_t bytes) {
   if (!p || bytes == 0) return true;
-  const uintptr_t page = 4096, lo = (uintptr_t)p & ~(page - 1), hi = ((uintptr_t)p + bytes + page - 1) & ~(page - 1);
+  const uintptr_t page = 4096;
+  uintptr_t lo = (uintptr_t)p & ~(page - 1), hi = ((uintptr_t)p + bytes + page - 1) & ~(page - 1);
   for (size_t i = 0; i < g->registered.size(); ++i) {
     auto e = g->registered[i];
     if (lo >= e.first && hi <= e.first + e.second) {
@@ -980,11 +988,20 @@ static bool ensure_registered(const void* p, size_t bytes) {
       return true;
     }
   }
-  // drop entries the new range overlaps (the caller re-used part of an old buffer) and the oldest beyond 16
+  // replace entries the new range overlaps (the caller re-used part of an old buffer, or a neighbour
+  // shares a page with it) by one registration of the union, so that the buffers they held stay
+  // covered; drop the oldest beyond 16
   for (size_t i = 0; i < g->registered.size();) {
     auto e = g->registered[i];
-    if (lo < e.first + e.second && e.first < hi) { cudaHostUnregister((void*)e.first); g->registered.erase(g->registered.begin() + i); }
-    else ++i;
+    if (lo < e.first + e.second && e.first < hi) {
+      cudaHostUnregister((void*)e.first);
+      g->registered.erase(g->registered.begin() + i);
+      lo = std::min(lo, e.first);
+      hi = std::max(hi, e.first + e.second);
+      i = 0; // the union may reach entries already passed
+    } else {
+      ++i;
+    }
   }
   while (g->registered.size() >= 16) { cudaHostUnregister((void*)g->registered.front().first); g->registered.erase(g->registered.begin()); }
   if (cudaHostRegister((void*)lo, hi - lo, cudaHostRegisterDefault) != cudaSuccess) { (void)cudaGetLastError(); return false; }
@@ -1017,13 +1034,12 @@ static int host_pipeline(const PipeSpec& sp) {
   const int n = g->ctrl.n, R = Ctx::kBounceSlots;
   const bool ag = sp.coll == B200MPI_COLL_ALLGATHER;
   const size_t rows = ag ? (size_t)n : 1;
-  bool pinned = is_pinned(sp.in) && is_pinned(sp.out);
+  const size_t in_bytes = sp.in ? B : 0, out_bytes = sp.out ? B * rows : 0;
+  bool pinned = is_pinned(sp.in, in_bytes) && is_pinned(sp.out, out_bytes);
   if (!pinned && g->host_register)
-    pinned = (is_pinned(sp.in) || ensure_registered(sp.in, sp.in ? B : 0)) && (is_pinned(sp.out) || ensure_registered(sp.out, sp.out ? B * rows : 0));
+    pinned = (is_pinned(sp.in, in_bytes) || ensure_registered(sp.in, in_bytes)) && (is_pinned(sp.out, out_bytes) || ensure_registered(sp.out, out_bytes));
   const bool bounce = !pinned && g->host_threads > 0;
-  size_t chunk_bytes = g->pipe_chunk_bytes;
-  if (bounce) chunk_bytes = std::min(chunk_bytes, g->bounce_chunk_bytes);
-  size_t chunk_elems = std::max<size_t>(chunk_bytes / rows / es, 4096) / 4096 * 4096;
+  const size_t chunk_elems = pipe_chunk_elems(es, rows, n, bounce, g->pipe_chunk_bytes, g->bounce_chunk_bytes);
   const size_t nch = (sp.count + chunk_elems - 1) / chunk_elems;
   int rc = ensure_stage(0, B);
   if (rc) return rc;

@@ -155,6 +155,18 @@ struct CopyPool {
   }
 };
 
+// Elements per chunk of a pipelined host-slice collective (b200mpi.cu: host_pipeline): a multiple of
+// 4096, at least 4096.  rows is n for Allgather (each chunk moves n rows), else 1.  In a multi-rank
+// world every chunk launch pairs with the launch of the same number on every peer, so the chunk may
+// only depend on what all ranks share: the knobs, the element size and n.  Whether this rank's
+// buffer is pinned, registered or bounced is its own business, and the smaller of the two knobs
+// serves all of them.  A world of one pairs nothing: a buffer that needs no bounce keeps the larger
+// pipe chunk there.
+static inline size_t pipe_chunk_elems(size_t es, size_t rows, int n, bool bounce, size_t pipe_chunk_bytes, size_t bounce_chunk_bytes) {
+  const size_t bytes = n > 1 || bounce ? std::min(pipe_chunk_bytes, bounce_chunk_bytes) : pipe_chunk_bytes;
+  return std::max<size_t>(bytes / rows / es, 4096) / 4096 * 4096;
+}
+
 // ---------------------------------------------------------------------------------------------
 // Counter settings read at Init.
 //   B200MPI_SCRUB_EVERY   launches between two flag scrubs: a power of two (rounded down, at least 2),

@@ -209,8 +209,8 @@ int b200mpi_set_max_blocks(int blocks); /* cap grid size (0 = default: SMs x occ
  * "allgather_nvls_min", "host_register" (pin pageable host slices in place, cached; 0 drops the cache),
  * "p2p_fast" (host-slice Send/Receive through mapped pinned buffers), "watchdog_ms". */
 int b200mpi_set_param(const char* name, int64_t value);
-/* Read only, besides the knobs above: "sm_count", "shared_device", "epoch" (the barrier epoch the next
- * launch takes) and "ll_seq" (the last LL Allreduce sequence number issued). */
+/* Reads every knob above, and these read-only values: "sm_count", "shared_device", "epoch" (the barrier
+ * epoch the next launch takes) and "ll_seq" (the last LL Allreduce sequence number issued). */
 int b200mpi_get_param(const char* name, int64_t* value);
 /* cudaStream_t used for collectives; set NULL to restore the library's own stream. */
 int b200mpi_get_stream(void** stream);

@@ -26,11 +26,13 @@
 #include <chrono>
 #include <condition_variable>
 #include <deque>
+#include <limits>
 #include <map>
 #include <mutex>
 #include <thread>
 #include <set>
 #include <string>
+#include <variant>
 #include <vector>
 
 #include "../../include/b200mpi.h"
@@ -132,20 +134,22 @@ struct Ctx {
   struct P2PBounce { char* host = nullptr; char* dev = nullptr; uint32_t seq = 0; bool busy = false; };
   P2PBounce p2p_bounce[kP2PBounces];
   std::mutex p2p_mu;
-  int p2p_fast = 1;
+  bool p2p_fast = true;
   // Opt-in (B200MPI_HOST_REGISTER=1 / "host_register"): pin the caller's pageable buffers in place
   // (cudaHostRegister, cached by address range) instead of bouncing them.  Only for callers whose
   // buffers stay mapped for the life of the cache (a freed and re-mapped range would alias stale
   // pinned pages); off by default.
-  int host_register = 0;
+  bool host_register = false;
   std::vector<std::pair<uintptr_t, size_t>> registered; // LRU, most recent last
   int gpu_numa_node = -1;      // NUMA node of the bound GPU (-1 unknown): host buffers and helper threads go there
   size_t oneshot_max_bytes = 256u << 10;
+  // Above a few MiB Bcast and Allgather stay on the P2P kernels, and the hybrid allreduce stays off,
+  // until multicast delivery has been measured against plain P2P stores on H100.
   int hybrid_p2p_permille = 0; // Allreduce HYBRID: share of the message that goes the P2P way, in 1/1000
   int hybrid_p2p_blocks = 0;   // CTAs given to the P2P part (0 = sm_count - nvls_max_blocks)
-  int bcast_nvls2 = 1;         // Bcast NVLS: scatter + multicast (1) or root-only multicast (0)
-  size_t bcast_nvls_min = 0, allgather_nvls_min = 0; // AUTO thresholds (bytes), set at init from n
-  int twoshot_unroll = 1; // 0: 1/2/4 vectors per thread for n = 8/4/2, 1: 2/4/8
+  bool bcast_nvls2 = true;     // Bcast NVLS: scatter + multicast (1) or root-only multicast (0)
+  size_t bcast_nvls_min = SIZE_MAX, allgather_nvls_min = SIZE_MAX; // AUTO thresholds (bytes)
+  bool twoshot_unroll = true; // 0: 1/2/4 vectors per thread for n = 8/4/2, 1: 2/4/8
   int nvls_unroll = 2;      // multi-GPU switch tuning: not yet measured on H100 (tools/sweep.py re-derives it)
   int nvls_max_blocks = 48; // fewer requests in flight suit the switch reduction; not yet measured on H100
   size_t ll_max_bytes = 0; // AUTO uses the barrier-free LL allreduce for messages up to this size (<= 256 KiB)
@@ -191,9 +195,11 @@ static size_t esize(int dtype) {
   return 0;
 }
 
+static int need_init() { return g && g->initialised ? 0 : fail(B200MPI_ERR_NOT_INIT, "mpi: Init has not been called"); }
+
 static thread_local int t_bound_dev = -1;
 static int need_data_plane() {
-  if (!g || !g->initialised) return fail(B200MPI_ERR_NOT_INIT, "mpi: Init has not been called");
+  if (int rc = need_init()) return rc;
   if (g->control_only) return fail(B200MPI_ERR_NO_DEVICE, "no CUDA device bound (control-plane-only init); there is no CPU data path");
   if (t_bound_dev != g->dev) { // the CUDA "current device" is per host thread; Send/Receive come from any goroutine/thread
     if (cudaSetDevice(g->dev) != cudaSuccess) return fail(B200MPI_ERR_CUDA, "cudaSetDevice failed on a caller thread");
@@ -1777,26 +1783,101 @@ int b200mpi_size(void) { return (g && g->initialised) ? g->ctrl.n : 0; }
 int b200mpi_device(void) { return (g && g->initialised && !g->control_only) ? g->dev : -1; }
 int64_t b200mpi_launch_count(void) { return g ? g->launches.load() : 0; }
 
-// Size thresholds of the AUTO policies (multi-GPU; not yet measured on H100).
-// Functions of n (and of whether the switch path exists) only, so every rank agrees.
-static void apply_defaults() {
-  const int n = g->ctrl.n;
-  const bool nvls = g->heap.mc_base != 0;
-  g->ll_max_bytes = 0;
-  // LL (no barrier, one exchange latency) over its whole range on real multi-GPU worlds
-  if (!g->shared_device) g->ll_max_bytes = std::min<size_t>(256u << 10, ll_cells(n) * 8);
-  // Above a few MiB Bcast and Allgather stay on the P2P kernels, and the hybrid allreduce stays off,
-  // until multicast delivery has been measured against plain P2P stores on H100.
-  g->bcast_nvls_min = SIZE_MAX;
-  g->allgather_nvls_min = SIZE_MAX;
-  g->hybrid_p2p_permille = 0;
-  // ranks time-slicing one GPU (functional-test mode): every extra kernel costs a time slice, keep the
-  // host-slice Send/Receive on the copy-engine path there
-  g->p2p_fast = g->shared_device ? 0 : 1;
-  if (const char* w = getenv("B200MPI_P2P_FAST")) g->p2p_fast = atoi(w) != 0;
-  (void)nvls;
-  if (const char* w = getenv("B200MPI_LL_MAX")) g->ll_max_bytes = std::min<size_t>(strtoull(w, nullptr, 0), ll_cells(g->ctrl.n) * 8);
-  if (const char* w = getenv("B200MPI_HYBRID_PERMILLE")) g->hybrid_p2p_permille = std::max(0, std::min(900, atoi(w)));
+// The tuning knobs of set_param / get_param, one row each; sm_count and the rows after it are read only.
+// The compiled-in defaults are the member initialisers of Ctx.
+using KnobField = std::variant<bool Ctx::*, int Ctx::*, uint32_t Ctx::*, int64_t Ctx::*, size_t Ctx::*>;
+constexpr int64_t kLaneCap = -1; // as hi: the world's LL lane capacity, ll_cells(n) * 8 (ll_max_bytes only)
+struct Knob {
+  const char* name;
+  KnobField field;                                   // holds value * scale (a bool holds value != 0)
+  const char* env = nullptr;                         // B200MPI_* variable that overrides the default at Init
+  int64_t lo = INT64_MIN, hi = INT64_MAX, scale = 1; // clamp, in set_param's units
+};
+static const Knob kKnobs[] = {
+    {"twoshot_unroll", &Ctx::twoshot_unroll},
+    {"nvls_unroll", &Ctx::nvls_unroll},
+    {"nvls_min_ranks", &Ctx::nvls_min_ranks},
+    {"nvls_max_blocks", &Ctx::nvls_max_blocks, nullptr, 1},
+    {"oneshot_max_bytes", &Ctx::oneshot_max_bytes, "B200MPI_ONESHOT_MAX"},
+    {"ll_max_bytes", &Ctx::ll_max_bytes, "B200MPI_LL_MAX", 0, kLaneCap},
+    {"stage_chunk", &Ctx::stage_chunk, "B200MPI_STAGE_CHUNK", 4096},
+    {"pipe_min_bytes", &Ctx::pipe_min_bytes},
+    {"pipe_chunk_bytes", &Ctx::pipe_chunk_bytes, nullptr, 65536},
+    {"bounce_chunk_bytes", &Ctx::bounce_chunk_bytes, nullptr, 65536},
+    {"host_threads", &Ctx::host_threads, "B200MPI_HOST_THREADS", 0},
+    {"own_block_bytes", &Ctx::own_block_bytes, nullptr, 4096},
+    {"hybrid_p2p_permille", &Ctx::hybrid_p2p_permille, "B200MPI_HYBRID_PERMILLE", 0, 900},
+    {"hybrid_p2p_blocks", &Ctx::hybrid_p2p_blocks, nullptr, 0},
+    {"hybrid_min_bytes", &Ctx::hybrid_min_bytes, nullptr, 0},
+    {"bcast_nvls2", &Ctx::bcast_nvls2},
+    {"bcast_nvls_min", &Ctx::bcast_nvls_min, nullptr, 0},
+    {"allgather_nvls_min", &Ctx::allgather_nvls_min, nullptr, 0},
+    {"host_register", &Ctx::host_register, "B200MPI_HOST_REGISTER"},
+    {"p2p_fast", &Ctx::p2p_fast, "B200MPI_P2P_FAST"},
+    {"watchdog_ms", &Ctx::watchdog_ns, nullptr, 1, INT64_MAX, 1000000},
+    {"sm_count", &Ctx::sm_count},
+    {"shared_device", &Ctx::shared_device},
+    {"epoch", &Ctx::epoch},
+    {"ll_seq", &Ctx::ll_seq},
+};
+static const Knob* find_knob(const char* name) {
+  for (const Knob& k : kKnobs) if (name && strcmp(name, k.name) == 0) return &k;
+  return nullptr;
+}
+// The one clamp of a knob, for set_param and the environment alike: the row's range, then what the field
+// holds, scaled.  A size_t field takes a negative value as its bit pattern, which get_param gives back.
+static void store_knob(const Knob& k, int64_t v) {
+  v = std::max(k.lo, std::min(v, k.hi == kLaneCap ? (int64_t)(ll_cells(g->ctrl.n) * 8) : k.hi));
+  std::visit([&](auto m) {
+    using T = std::remove_reference_t<decltype(g->*m)>;
+    constexpr bool narrow = sizeof(T) < sizeof(int64_t);
+    const int64_t tlo = narrow ? (int64_t)std::numeric_limits<T>::min() : INT64_MIN;
+    const int64_t thi = narrow ? (int64_t)std::numeric_limits<T>::max() : INT64_MAX;
+    if constexpr (std::is_same_v<T, bool>) g->*m = v != 0;
+    else g->*m = (T)(std::clamp(v, tlo / k.scale, thi / k.scale) * k.scale);
+  }, k.field);
+}
+// Init's last word on the knobs.  First the defaults that follow from the world: functions of n and
+// of shared_device only, so every rank agrees.  Then every B200MPI_* override, through the clamp.
+static void settle_knobs() {
+  if (!g->control_only) {
+    // LL (no barrier, one exchange latency) over its whole range on real multi-GPU worlds
+    if (!g->shared_device) g->ll_max_bytes = std::min<size_t>(256u << 10, ll_cells(g->ctrl.n) * 8);
+    // ranks time-slicing one GPU (functional-test mode): every extra kernel costs a time slice, keep the
+    // host-slice Send/Receive on the copy-engine path there
+    g->p2p_fast = !g->shared_device;
+  }
+  for (const Knob& k : kKnobs)
+    if (const char* w = k.env ? getenv(k.env) : nullptr) store_knob(k, strtoll(w, nullptr, 0));
+}
+// Unregisters the host_register cache after the copies that may use it; no CUDA call when it is empty.
+static void drop_registrations() {
+  if (g->registered.empty()) return;
+  cudaStreamSynchronize(g->h2d_stream);
+  cudaStreamSynchronize(g->d2h_stream);
+  for (auto& e : g->registered) cudaHostUnregister((void*)e.first);
+  g->registered.clear();
+  (void)cudaGetLastError();
+}
+// Releases everything a Ctx owns and deletes it, each release guarded, so it also undoes a partial Init.
+static void teardown() {
+  drop_registrations(); // while the copy streams it synchronises still exist
+  for (cudaStream_t s : g->stream_pool) cudaStreamDestroy(s);
+  for (cudaStream_t s : {g->own_stream, g->h2d_stream, g->d2h_stream}) if (s) cudaStreamDestroy(s);
+  for (cudaEvent_t e : g->pipe_events) cudaEventDestroy(e);
+  for (cudaEvent_t e : {g->ev0, g->ev1}) if (e) cudaEventDestroy(e);
+  if (g->pool.running()) g->pool.shutdown(); // its threads fill the bounce ring
+  for (void* p : {(void*)g->bounce, (void*)g->status_host, (void*)g->ll_host}) if (p) cudaFreeHost(p);
+  for (auto& b : g->p2p_bounce) if (b.host) cudaFreeHost(b.host);
+  if (g->box) munmap(g->box, sizeof(Mailbox));
+  {
+    std::lock_guard<std::mutex> l(g_pending_mu);
+    g_pending.clear();
+  }
+  g->heap.destroy(g->drv); // no-op when the heap was never created
+  g->ctrl.shutdown();
+  delete g;
+  g = nullptr;
 }
 
 // Test hook (B200MPI_EPOCH_START = e): give this rank's control region the state of a long-running job
@@ -1829,24 +1910,11 @@ int b200mpi_init(const char* addr, const char* alladdr_csv, const char* password
   int rc = g->ctrl.init(addr, alladdr_csv, password, timeout_ns, err);
   if (rc) { delete g; g = nullptr; return fail(rc, err); }
   if (const char* w = getenv("B200MPI_WATCHDOG_S")) g->watchdog_ns = (int64_t)(atof(w) * 1e9);
-  if (const char* w = getenv("B200MPI_STAGE_CHUNK")) g->stage_chunk = std::max<size_t>(strtoull(w, nullptr, 0), 4096);
-  if (const char* w = getenv("B200MPI_ONESHOT_MAX")) g->oneshot_max_bytes = strtoull(w, nullptr, 0);
-  auto bail = [&](int code, const std::string& m) {
-    // tell nobody: peers notice through their own control-plane errors / timeouts
-    if (g->box) munmap(g->box, sizeof(Mailbox));
-    if (g->status_host) cudaFreeHost(g->status_host);
-    for (cudaStream_t st : {g->own_stream, g->h2d_stream, g->d2h_stream})
-      if (st) cudaStreamDestroy(st);
-    if (g->ev0) cudaEventDestroy(g->ev0);
-    if (g->ev1) cudaEventDestroy(g->ev1);
-    if (g->drv.MemUnmap) g->heap.destroy(g->drv); // no-op when the heap was never created
-    g->ctrl.shutdown();
-    delete g;
-    g = nullptr;
-    return fail(code, m);
-  };
+  // tell nobody: peers notice through their own control-plane errors / timeouts
+  auto bail = [&](int code, const std::string& m) { teardown(); return fail(code, m); };
   if (gpu == -2) {
     g->control_only = true;
+    settle_knobs();
     g->initialised = true;
     return 0;
   }
@@ -1872,8 +1940,6 @@ int b200mpi_init(const char* addr, const char* alladdr_csv, const char* password
   g->scrub_every = cenv.scrub_every;
   g->epoch = cenv.epoch_start;
   g->ll_seq = cenv.ll_seq_start;
-  if (const char* w = getenv("B200MPI_HOST_THREADS")) g->host_threads = std::max(0, atoi(w));
-  if (const char* w = getenv("B200MPI_HOST_REGISTER")) g->host_register = atoi(w) != 0;
 
   // who sits where: ranks sharing a device (functional-test mode) rule out NVLS.  The counter settings
   // travel along: ranks that disagree on them (or a rank that could not parse them) fail Init on every
@@ -1946,7 +2012,7 @@ int b200mpi_init(const char* addr, const char* alladdr_csv, const char* password
   g->comm.timeout_ns = (unsigned long long)g->watchdog_ns;
   g->comm.rank = g->ctrl.rank;
   g->comm.n = g->ctrl.n;
-  apply_defaults();
+  settle_knobs();
   if (cenv.preset && preset_control_region(cenv.epoch_start)) return bail(B200MPI_ERR_CUDA, t_err);
   rc = g->ctrl.barrier(err);
   if (rc) return bail(rc, err);
@@ -1963,30 +2029,7 @@ int b200mpi_finalize(void) {
     cudaDeviceSynchronize();
   }
   g->ctrl.barrier(err); // nobody unmaps while a peer may still read
-  if (!g->control_only) {
-    for (cudaStream_t s : g->stream_pool) cudaStreamDestroy(s);
-    if (g->own_stream) cudaStreamDestroy(g->own_stream);
-    if (g->h2d_stream) cudaStreamDestroy(g->h2d_stream);
-    if (g->d2h_stream) cudaStreamDestroy(g->d2h_stream);
-    for (cudaEvent_t e : g->pipe_events) cudaEventDestroy(e);
-    if (g->ev0) cudaEventDestroy(g->ev0);
-    if (g->ev1) cudaEventDestroy(g->ev1);
-    if (g->status_host) cudaFreeHost(g->status_host);
-    if (g->ll_host) cudaFreeHost(g->ll_host);
-    for (auto& b : g->p2p_bounce) if (b.host) cudaFreeHost(b.host);
-    if (g->pool.running()) g->pool.shutdown();
-    if (g->bounce) cudaFreeHost(g->bounce);
-    for (auto& e : g->registered) cudaHostUnregister((void*)e.first);
-    if (g->box) munmap(g->box, sizeof(Mailbox));
-    {
-      std::lock_guard<std::mutex> l(g_pending_mu);
-      g_pending.clear();
-    }
-    g->heap.destroy(g->drv);
-  }
-  g->ctrl.shutdown();
-  delete g;
-  g = nullptr;
+  teardown();
   return 0;
 }
 
@@ -2174,7 +2217,7 @@ int b200mpi_stream_sync(void) {
 }
 
 int b200mpi_barrier(void) {
-  if (!g || !g->initialised) return fail(B200MPI_ERR_NOT_INIT, "mpi: Init has not been called");
+  if (int rc = need_init()) return rc;
   if (g->control_only) {
     std::string err;
     int rc = g->ctrl.barrier(err);
@@ -2187,7 +2230,7 @@ int b200mpi_barrier(void) {
 }
 
 int b200mpi_set_algo(int coll, int algo) {
-  if (!g || !g->initialised) return fail(B200MPI_ERR_NOT_INIT, "mpi: Init has not been called");
+  if (int rc = need_init()) return rc;
   if (coll < 0 || coll > B200MPI_COLL_REDUCE_SCATTER || algo < 0 || algo > B200MPI_ALGO_HYBRID) return fail(B200MPI_ERR_ARG, "set_algo: bad collective or algorithm id");
   g->algo[coll] = algo;
   return 0;
@@ -2203,74 +2246,27 @@ int b200mpi_get_algo(int coll, size_t count, int dtype) {
   return fail(B200MPI_ERR_ARG, "get_algo: bad collective id");
 }
 int b200mpi_set_param(const char* name, int64_t value) {
-  if (!g || !g->initialised) return fail(B200MPI_ERR_NOT_INIT, "mpi: Init has not been called");
-  std::string k = name ? name : "";
-  if (k == "twoshot_unroll") g->twoshot_unroll = value ? 1 : 0;
-  else if (k == "nvls_unroll") g->nvls_unroll = (int)value;
-  else if (k == "nvls_min_ranks") g->nvls_min_ranks = (int)value;
-  else if (k == "ll_max_bytes") g->ll_max_bytes = (size_t)std::min<int64_t>(std::max<int64_t>(value, 0), (int64_t)(ll_cells(g->ctrl.n) * 8));
-  else if (k == "nvls_max_blocks") g->nvls_max_blocks = (int)std::max<int64_t>(1, value);
-  else if (k == "oneshot_max_bytes") g->oneshot_max_bytes = (size_t)value;
-  else if (k == "pipe_min_bytes") g->pipe_min_bytes = (size_t)value;
-  else if (k == "pipe_chunk_bytes") g->pipe_chunk_bytes = (size_t)std::max<int64_t>(value, 65536);
-  else if (k == "own_block_bytes") g->own_block_bytes = (size_t)std::max<int64_t>(value, 4096);
-  else if (k == "stage_chunk") g->stage_chunk = (size_t)std::max<int64_t>(value, 4096);
-  else if (k == "watchdog_ms") { g->watchdog_ns = std::max<int64_t>(value, 1) * 1000000ll; g->comm.timeout_ns = (unsigned long long)g->watchdog_ns; }
-  else if (k == "hybrid_p2p_permille") g->hybrid_p2p_permille = (int)std::min<int64_t>(std::max<int64_t>(value, 0), 900);
-  else if (k == "hybrid_p2p_blocks") g->hybrid_p2p_blocks = (int)std::max<int64_t>(value, 0);
-  else if (k == "hybrid_min_bytes") g->hybrid_min_bytes = (size_t)std::max<int64_t>(value, 0);
-  else if (k == "bcast_nvls2") g->bcast_nvls2 = value ? 1 : 0;
-  else if (k == "bcast_nvls_min") g->bcast_nvls_min = (size_t)std::max<int64_t>(value, 0);
-  else if (k == "allgather_nvls_min") g->allgather_nvls_min = (size_t)std::max<int64_t>(value, 0);
-  else if (k == "host_register") {
-    g->host_register = value ? 1 : 0;
-    if (!value) { // leaving the mode drops every cached registration: the caller may free those buffers now
-      cudaStreamSynchronize(g->h2d_stream);
-      cudaStreamSynchronize(g->d2h_stream);
-      for (auto& e : g->registered) cudaHostUnregister((void*)e.first);
-      g->registered.clear();
-      (void)cudaGetLastError();
-    }
-  }
-  else if (k == "p2p_fast") g->p2p_fast = value ? 1 : 0;
-  else if (k == "bounce_chunk_bytes") g->bounce_chunk_bytes = (size_t)std::max<int64_t>(value, 65536);
-  else if (k == "host_threads") { if (g->pool.running()) return fail(B200MPI_ERR_ARG, "set_param: host_threads must be set before the first pageable host-slice call"); g->host_threads = (int)std::max<int64_t>(value, 0); }
-  else return fail(B200MPI_ERR_ARG, "set_param: unknown parameter '" + k + "'");
+  if (int rc = need_init()) return rc;
+  const Knob* k = find_knob(name);
+  if (!k || k >= find_knob("sm_count")) return fail(B200MPI_ERR_ARG, std::string("set_param: unknown parameter '") + (name ? name : "") + "'");
+  if (k->field == KnobField(&Ctx::host_threads) && g->pool.running())
+    return fail(B200MPI_ERR_ARG, "set_param: host_threads must be set before the first pageable host-slice call");
+  store_knob(*k, value);
+  if (k->field == KnobField(&Ctx::watchdog_ns)) g->comm.timeout_ns = (unsigned long long)g->watchdog_ns;
+  // leaving host_register mode drops every cached registration: the caller may free those buffers now
+  if (k->field == KnobField(&Ctx::host_register) && !g->host_register) drop_registrations();
   return 0;
 }
 int b200mpi_get_param(const char* name, int64_t* value) {
-  if (!g || !g->initialised) return fail(B200MPI_ERR_NOT_INIT, "mpi: Init has not been called");
+  if (int rc = need_init()) return rc;
   if (!value) return fail(B200MPI_ERR_ARG, "get_param: NULL result pointer");
-  const std::string k = name ? name : "";
-  if (k == "twoshot_unroll") *value = g->twoshot_unroll;
-  else if (k == "nvls_unroll") *value = g->nvls_unroll;
-  else if (k == "nvls_min_ranks") *value = g->nvls_min_ranks;
-  else if (k == "nvls_max_blocks") *value = g->nvls_max_blocks;
-  else if (k == "ll_max_bytes") *value = (int64_t)g->ll_max_bytes;
-  else if (k == "oneshot_max_bytes") *value = (int64_t)g->oneshot_max_bytes;
-  else if (k == "pipe_min_bytes") *value = (int64_t)g->pipe_min_bytes;
-  else if (k == "pipe_chunk_bytes") *value = (int64_t)g->pipe_chunk_bytes;
-  else if (k == "bounce_chunk_bytes") *value = (int64_t)g->bounce_chunk_bytes;
-  else if (k == "host_threads") *value = g->host_threads;
-  else if (k == "host_register") *value = g->host_register;
-  else if (k == "own_block_bytes") *value = (int64_t)g->own_block_bytes;
-  else if (k == "stage_chunk") *value = (int64_t)g->stage_chunk;
-  else if (k == "watchdog_ms") *value = g->watchdog_ns / 1000000ll;
-  else if (k == "hybrid_p2p_permille") *value = g->hybrid_p2p_permille;
-  else if (k == "hybrid_p2p_blocks") *value = g->hybrid_p2p_blocks;
-  else if (k == "hybrid_min_bytes") *value = (int64_t)g->hybrid_min_bytes;
-  else if (k == "bcast_nvls2") *value = g->bcast_nvls2;
-  else if (k == "bcast_nvls_min") *value = (int64_t)g->bcast_nvls_min;
-  else if (k == "allgather_nvls_min") *value = (int64_t)g->allgather_nvls_min;
-  else if (k == "sm_count") *value = g->sm_count;
-  else if (k == "shared_device") *value = g->shared_device ? 1 : 0;
-  else if (k == "epoch") *value = (int64_t)g->epoch;
-  else if (k == "ll_seq") *value = (int64_t)g->ll_seq;
-  else return fail(B200MPI_ERR_ARG, "get_param: unknown parameter '" + k + "'");
+  const Knob* k = find_knob(name);
+  if (!k) return fail(B200MPI_ERR_ARG, std::string("get_param: unknown parameter '") + (name ? name : "") + "'");
+  *value = std::visit([&](auto m) { return (int64_t)(g->*m) / k->scale; }, k->field);
   return 0;
 }
 int b200mpi_set_max_blocks(int blocks) {
-  if (!g || !g->initialised) return fail(B200MPI_ERR_NOT_INIT, "mpi: Init has not been called");
+  if (int rc = need_init()) return rc;
   if (blocks < 0 || blocks > kMaxBlocks) return fail(B200MPI_ERR_ARG, "set_max_blocks: out of range");
   g->max_blocks = blocks; // block_cap() clamps to the SM count: the cross-rank barriers need every CTA resident
   return 0;

@@ -154,7 +154,7 @@ class Guarded:
         if body is not None:
             self.set_body(body)
         if kind == "heap":
-            self.mem = mpi.Alloc(self.total, np.uint8).copy_from_host(self.image)
+            self.mem = self.alloc(self.total).copy_from_host(self.image)
             self.view = mpi.DeviceSlice(self.count, self.dt, self.mem.ptr + self.head, owner=False)
         else:
             raw = np.empty(self.total + 64, dtype=np.uint8)
@@ -162,6 +162,10 @@ class Guarded:
             self.mem = raw[s:s + self.total]
             self.mem[:] = self.image
             self.view = self.mem[self.head:self.head + self.nbody].view(self.dt)
+
+    def alloc(self, nbytes):
+        """The heap allocation behind a 'heap' buffer."""
+        return mpi.Alloc(nbytes, np.uint8)
 
     def set_body(self, arr, lo=0):
         """The elements from `lo` on must hold `arr` after the call."""
@@ -533,13 +537,14 @@ def part_bytes(R):
                 do_alltoall(R, dn, count, layout, R.kind_for(ci + li + di, count * n * es))
 
 
-def part_v(R):
+def part_v(R, counts=None, skew=None):
     """Gatherv and Scatterv (through the C ABI, so that every rank passes both buffers), Allgatherv and
-    Alltoallv on skewed tables."""
+    Alltoallv on skewed tables (counts and skew, when given, replace the default tables)."""
     lib, rank, n = R.lib, R.rank, R.n
-    counts = v_tables(n)[4]  # one rank carries 70001 elements, the others 5 + r
-    skew = dict(AV.tables(n, SEED))["one pair"]
-    if R.trim == "edges":
+    given = counts is not None
+    counts = counts if given else v_tables(n)[4]  # one rank carries 70001 elements, the others 5 + r
+    skew = skew if skew is not None else dict(AV.tables(n, SEED))["one pair"]
+    if R.trim == "edges" and not given:
         counts = [c if c < 1000 else 4099 for c in counts]
         skew = [[c if c < 1000 else 4099 for c in row] for row in skew]
     total = sum(counts)

@@ -125,11 +125,17 @@ int b200mpi_send(const void* buf, size_t count, int dtype, int dest, int tag, in
 /* The Send/Wait pair sketched in the reference (mpi.go:132-152, commented out there): isend
  * returns once the data has left the caller's buffer ("sent on connection", here: staged in this
  * rank's device heap), without waiting for the receiver; wait blocks until `dest` confirmed the
- * message with `tag` and frees the {dest, tag} pair.  Every isend must be followed by one wait. */
+ * message with `tag` and frees the {dest, tag} pair.  Every isend must be followed by one wait.
+ * Each (rank, dest) pair has 16 mailbox slots; a send holds one until it returns, an isend until its
+ * wait, whether or not the message was received.  So at most 16 isends to one dest may be unwaited:
+ * the 17th finds no free slot and fails with B200MPI_ERR_TIMEOUT after the watchdog time. */
 int b200mpi_isend(const void* buf, size_t count, int dtype, int dest, int tag, int memkind);
 int b200mpi_wait(int dest, int tag);
 /* Blocks for message (src, tag).  *count_out = elements sent (gob resizes the destination,
- * network.go:597); more than `capacity` elements => B200MPI_ERR_TRUNCATE, *count_out = needed. */
+ * network.go:597); more than `capacity` elements => B200MPI_ERR_TRUNCATE, *count_out = needed.
+ * A host buffer is filled through a staging block of at most "stage_chunk" bytes (32 MiB) in this
+ * rank's heap, whatever memory the sender passed; without room for it => B200MPI_ERR_NOMEM.  After
+ * either error nothing is written and the message stays posted: receive it again. */
 int b200mpi_recv(void* buf, size_t capacity, size_t* count_out, int dtype, int src, int tag,
                  int memkind);
 

@@ -1725,28 +1725,35 @@ static int do_recv(void* buf, size_t capacity, size_t* count_out, int dtype, int
   // message lies contiguous in the sender's heap), is pulled whole once all of it is posted: ONE
   // kernel moves it over NVLink straight into a mapped pinned bounce (the SMs write host memory),
   // then a memcpy.  Otherwise each chunk is pulled as soon as it is posted, into a device buffer
-  // directly, or through a staging block and a D2H copy into a host slice.
-  const size_t nreg = slot->nregions ? slot->nregions : 1;
+  // directly, or through a staging block and a D2H copy into a host slice.  That staging block is
+  // at most this rank's stage_chunk, whatever the sender's layout: a chunk larger than that (a direct
+  // post or an Isend is one chunk of the whole message) is pulled in several units, so that the heap a
+  // host receive needs does not depend on the memory the sender passed.
+  const size_t nreg = slot->nregions ? slot->nregions : 1, chunk = slot->chunk_bytes;
   Ctx::P2PBounce* bounce = nullptr;
-  if (rc == 0 && bytes && memkind == B200MPI_HOST && g->p2p_fast && slot->chunk_bytes * nreg >= bytes && bytes <= Ctx::kP2PBounceBytes) bounce = acquire_bounce();
-  const size_t unit = bounce ? bytes : slot->chunk_bytes;
+  if (rc == 0 && bytes && memkind == B200MPI_HOST && g->p2p_fast && chunk * nreg >= bytes && bytes <= Ctx::kP2PBounceBytes) bounce = acquire_bounce();
+  const size_t unit = bounce ? bytes : memkind == B200MPI_HOST ? std::min(chunk, g->stage_chunk) : chunk;
   size_t stage = 0;
-  bool staged = false;
-  if (rc == 0 && bytes && !bounce && memkind == B200MPI_HOST) {
-    if (g->heap.alloc(unit, stage)) rc = fail(B200MPI_ERR_NOMEM, "recv: symmetric heap exhausted while staging");
-    else staged = true;
+  const bool staged = rc == 0 && bytes && !bounce && memkind == B200MPI_HOST;
+  if (staged && g->heap.alloc(unit, stage)) {
+    // Nothing is consumed, as for a truncation: the message stays posted, so the caller can free heap
+    // memory and receive it again.
+    slot->state.store(kPosted, std::memory_order_release);
+    return fail(B200MPI_ERR_NOMEM, "recv: symmetric heap exhausted while staging " + std::to_string(unit) + " bytes (raise B200MPI_HEAP_BYTES or lower stage_chunk)");
   }
   cudaStream_t s = rc == 0 && bytes ? borrow_stream() : nullptr;
   const char* peer = (const char*)g->heap.base[src];
   char* mine = (char*)g->heap.base[me];
-  for (size_t lo = 0; rc == 0 && lo < bytes; lo += unit) {
-    // the sender publishes `posted` only at the end of a chunk
-    const size_t len = std::min(unit, bytes - lo);
+  for (size_t lo = 0, len = 0; rc == 0 && lo < bytes; lo += len) {
+    // The sender publishes `posted` only at the end of a chunk, and reuses a region once `done` has
+    // passed the end of its chunk: a unit never crosses a chunk's end (the bounce's one unit is the
+    // whole message, contiguous in the sender's heap).
+    len = bounce ? bytes : std::min({unit, chunk - lo % chunk, bytes - lo});
     Spinner sp(g->watchdog_ns);
     while (slot->posted.load(std::memory_order_acquire) < lo + len)
       if (!sp.step()) { rc = fail(B200MPI_ERR_TIMEOUT, "recv: sender stalled"); break; }
     if (rc) break;
-    const char* from = peer + slot->region_off[lo / unit % nreg];
+    const char* from = peer + slot->region_off[lo / chunk % nreg] + lo % chunk;
     cudaError_t e = cudaSuccess;
     if (bounce) {
       rc = copy_and_wait(bounce, bounce->dev, from, len, s);

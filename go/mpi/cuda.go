@@ -50,14 +50,22 @@ type DeviceSlice struct {
 	Ptr   unsafe.Pointer
 	Len   int
 	dtype C.int
+	loc   bool // elements are value-location pairs of dtype values (AllreduceLoc and ReduceLoc only)
 }
 
 // Alloc returns a device slice of n elements shaped like the zero-length prototype, e.g.
-// mpi.Alloc([]float32(nil), 1<<26).
+// mpi.Alloc([]float32(nil), 1<<26), or mpi.Alloc([]Float64Loc(nil), n) for the pairs of AllreduceLoc.
 func Alloc(prototype interface{}, n int) (*DeviceSlice, error) {
 	var dt C.int
 	var es int
+	loc := false
 	switch prototype.(type) {
+	case []Float32Loc:
+		dt, es, loc = dtF32, 16, true
+	case []Float64Loc:
+		dt, es, loc = dtF64, 16, true
+	case []Int64Loc:
+		dt, es, loc = dtI64, 16, true
 	case []float32:
 		dt, es = dtF32, 4
 	case []float64:
@@ -73,7 +81,7 @@ func Alloc(prototype interface{}, n int) (*DeviceSlice, error) {
 	if rc := C.b200mpi_alloc(C.size_t(n*es), &p); rc != 0 {
 		return nil, lastError(rc, 0)
 	}
-	return &DeviceSlice{Ptr: p, Len: n, dtype: dt}, nil
+	return &DeviceSlice{Ptr: p, Len: n, dtype: dt, loc: loc}, nil
 }
 
 // Free returns the slice to the heap.
@@ -124,6 +132,9 @@ func (c *Cuda) Size() int { return int(C.b200mpi_size()) }
 func lower(data interface{}) (unsafe.Pointer, int, C.int, C.int, error) {
 	switch v := data.(type) {
 	case *DeviceSlice:
+		if v.loc {
+			return nil, 0, 0, 0, errPairSlice
+		}
 		return v.Ptr, v.Len, v.dtype, C.B200MPI_DEVICE, nil
 	case []float64:
 		return ptr(len(v), func() unsafe.Pointer { return unsafe.Pointer(&v[0]) }), len(v), dtF64, C.B200MPI_HOST, nil
@@ -143,6 +154,8 @@ func lower(data interface{}) (unsafe.Pointer, int, C.int, C.int, error) {
 	b := buf.Bytes()
 	return ptr(len(b), func() unsafe.Pointer { return unsafe.Pointer(&b[0]) }), len(b), dtU8, C.B200MPI_HOST, nil
 }
+
+var errPairSlice = errors.New("mpi: a *DeviceSlice of value-location pairs goes through AllreduceLoc and ReduceLoc only")
 
 func ptr(n int, f func() unsafe.Pointer) unsafe.Pointer {
 	if n == 0 {
@@ -191,6 +204,9 @@ func recvBytes(buf []byte, source, tag int) ([]byte, error) {
 func (c *Cuda) Receive(data interface{}, source, tag int) error {
 	switch v := data.(type) {
 	case *DeviceSlice:
+		if v.loc {
+			return errPairSlice
+		}
 		n, rc := recvOnce(v.Ptr, v.Len, v.dtype, C.B200MPI_DEVICE, source, tag)
 		if rc != 0 {
 			return lastError(rc, tag)
@@ -682,6 +698,67 @@ func (c *Cuda) ReduceScatterv(send, recv interface{}, counts []int, op Op) ([]in
 		return nil, lastError(rc, 0)
 	}
 	return counts, nil
+}
+
+// lowerLoc turns a pair slice (or a *DeviceSlice allocated with a pair prototype) into (pointer,
+// pair count, dtype of the value, memkind). A nil slice is legal and lowers to a NULL pointer.
+func lowerLoc(what string, data interface{}) (unsafe.Pointer, int, C.int, C.int, error) {
+	switch v := data.(type) {
+	case *DeviceSlice:
+		if !v.loc {
+			return nil, 0, 0, 0, fmt.Errorf("mpi: %s needs a *DeviceSlice of pairs (Alloc([]Float64Loc(nil), n))", what)
+		}
+		return v.Ptr, v.Len, v.dtype, C.B200MPI_DEVICE, nil
+	case []Float32Loc:
+		return ptr(len(v), func() unsafe.Pointer { return unsafe.Pointer(&v[0]) }), len(v), dtF32, C.B200MPI_HOST, nil
+	case []Float64Loc:
+		return ptr(len(v), func() unsafe.Pointer { return unsafe.Pointer(&v[0]) }), len(v), dtF64, C.B200MPI_HOST, nil
+	case []Int64Loc:
+		return ptr(len(v), func() unsafe.Pointer { return unsafe.Pointer(&v[0]) }), len(v), dtI64, C.B200MPI_HOST, nil
+	}
+	return nil, 0, 0, 0, fmt.Errorf("mpi: %s takes []Float32Loc, []Float64Loc, []Int64Loc or a *DeviceSlice of them, got %T", what, data)
+}
+
+// AllreduceLoc: MAXLOC (Max) / MINLOC (Min) over pairs, in rank order, into every rank's recv.
+func (c *Cuda) AllreduceLoc(send, recv interface{}, op Op) error {
+	sp, sn, sdt, sk, err := lowerLoc("AllreduceLoc", send)
+	if err != nil {
+		return err
+	}
+	rp, rn, rdt, rk, err := lowerLoc("AllreduceLoc", recv)
+	if err != nil {
+		return err
+	}
+	if sn != rn || sdt != rdt || sk != rk {
+		return errors.New("mpi: AllreduceLoc send and recv must have the same length, pair type and memory kind")
+	}
+	if rc := C.b200mpi_allreduce_loc(sp, rp, C.size_t(sn), sdt, C.int(op), sk); rc != 0 {
+		return lastError(rc, 0)
+	}
+	return nil
+}
+
+// ReduceLoc: AllreduceLoc into root's recv only; recv may be nil elsewhere.
+func (c *Cuda) ReduceLoc(send, recv interface{}, op Op, root int) error {
+	sp, sn, sdt, sk, err := lowerLoc("ReduceLoc", send)
+	if err != nil {
+		return err
+	}
+	var rp unsafe.Pointer
+	if recv != nil {
+		var rn int
+		var rdt, rk C.int
+		if rp, rn, rdt, rk, err = lowerLoc("ReduceLoc", recv); err != nil {
+			return err
+		}
+		if sn != rn || sdt != rdt || sk != rk {
+			return errors.New("mpi: ReduceLoc send and recv must have the same length, pair type and memory kind")
+		}
+	}
+	if rc := C.b200mpi_reduce_loc(sp, rp, C.size_t(sn), sdt, C.int(op), C.int(root), sk); rc != 0 {
+		return lastError(rc, 0)
+	}
+	return nil
 }
 
 // Scatterv: root always sends its table with one small Bcast, so the other ranks may pass nil.

@@ -29,6 +29,7 @@
 //	Alltoallv                         Alltoall with a different length for every (source, destination) pair
 //	Scan, Exscan                      prefix reductions in rank order (inclusive, exclusive)
 //	ReduceScatterv                    ReduceScatter with a different block length for every rank
+//	AllreduceLoc, ReduceLoc           MAXLOC / MINLOC: the best value across ranks and where it came from
 //	Isend + Wait   the non-blocking Send design the reference sketches and comments out (mpi.go:132-152)
 //
 // They are served through the optional Collective interface, the upgrade the reference hints at
@@ -100,6 +101,31 @@ type Collective5 interface {
 // Collective6 is the sixth optional upgrade: the reduce-scatter whose blocks follow a counts table.
 type Collective6 interface {
 	ReduceScatterv(send, recv interface{}, counts []int, op Op) ([]int, error)
+}
+
+// Collective7 is the seventh optional upgrade: the value-location reductions (MPI's MAXLOC and
+// MINLOC). op is Max or Min.
+type Collective7 interface {
+	AllreduceLoc(send, recv interface{}, op Op) error
+	ReduceLoc(send, recv interface{}, op Op, root int) error
+}
+
+// Float32Loc, Float64Loc and Int64Loc are the elements of AllreduceLoc and ReduceLoc: a value and
+// where it came from. Each is 16 bytes, the layout of the C struct { V val; int64_t loc; } (4
+// padding bytes follow a float32).
+type Float32Loc struct {
+	Val float32
+	Loc int64
+}
+
+type Float64Loc struct {
+	Val float64
+	Loc int64
+}
+
+type Int64Loc struct {
+	Val int64
+	Loc int64
 }
 
 // Raw marks a payload that is sent as bytes without any encoding.
@@ -372,4 +398,35 @@ func ReduceScatterv(send, recv interface{}, counts []int, op Op) ([]int, error) 
 		return nil, fmt.Errorf("mpi: registered implementation %T has no ReduceScatterv", current)
 	}
 	return c.ReduceScatterv(send, recv, counts, op)
+}
+
+func collective7(what string) (Collective7, error) {
+	if c, ok := current.(Collective7); ok {
+		return c, nil
+	}
+	return nil, fmt.Errorf("mpi: registered implementation %T has no %s", current, what)
+}
+
+// AllreduceLoc combines, pair by pair and in rank order, every rank's send ([]Float32Loc,
+// []Float64Loc or []Int64Loc) into every rank's recv, a slice of the same type and length (it may be
+// send). With op Max (MAXLOC) or Min (MINLOC) a higher rank's pair replaces the running one when its
+// value is better, or equal with a smaller Loc. Floats compare as IEEE (-0 == +0), except that NaN is
+// better than every number under both ops and equal to every NaN, so NaN propagates as it does with
+// math.Max and math.Min. The winning pair is copied whole, so every rank gets the same bytes. Loc is
+// usually Rank() or a global index: a MINLOC with Loc = Rank() names the rank to Bcast from.
+func AllreduceLoc(send, recv interface{}, op Op) error {
+	c, err := collective7("AllreduceLoc")
+	if err != nil {
+		return err
+	}
+	return c.AllreduceLoc(send, recv, op)
+}
+
+// ReduceLoc is AllreduceLoc whose result lands in root's recv only; recv may be nil elsewhere.
+func ReduceLoc(send, recv interface{}, op Op, root int) error {
+	c, err := collective7("ReduceLoc")
+	if err != nil {
+		return err
+	}
+	return c.ReduceLoc(send, recv, op, root)
 }

@@ -32,7 +32,7 @@ extern "C" {
 
 #define B200MPI_VERSION 200 /* 0.2.0: + isend/wait, reduce_scatter, reduce, alltoall, probes, get_param;
                                then gather, scatter, gatherv, scatterv, allgatherv, alltoallv, scan, exscan,
-                               reduce_scatterv (all additive) */
+                               reduce_scatterv, allreduce_loc, reduce_loc (all additive) */
 #define B200MPI_MAX_RANKS 8 /* "the 8 GPUs of one box" */
 
 typedef enum {
@@ -194,6 +194,19 @@ int b200mpi_exscan(const void* send, void* recv, size_t count, int dtype, int op
  * send + displ[rank()] (the form in-place Allgatherv completes).  Buffers outside the b200mpi_alloc
  * heap are staged whole through it (B200MPI_ERR_NOMEM if too big). */
 int b200mpi_reduce_scatterv(const void* send, void* recv, const size_t* counts, int dtype, int op, int memkind);
+/* Value-location reductions (MPI_MAXLOC / MPI_MINLOC).  An element is the 16-byte pair
+ * struct { V val; int64_t loc; } with V = f32, f64 or i64 named by dtype (4 padding bytes follow an
+ * f32 value); count counts pairs.  op B200MPI_MAX is MAXLOC, B200MPI_MIN is MINLOC (SUM and u8:
+ * B200MPI_ERR_UNSUPPORTED).  Pairs are combined in rank order: a higher rank's pair replaces the
+ * running one when its value is better, or equal with a smaller loc (signed).  Floats compare as
+ * IEEE (-0 == +0), except that a NaN is better than every number for both ops and equal to every
+ * NaN, so NaN propagates (MPI leaves NaN undefined).  The winning pair is copied whole, padding
+ * included; of pairs equal in value and loc the lowest rank's wins, so the result does not depend on
+ * the algorithm.  Buffers must be 8-byte aligned (B200MPI_ERR_ARG).  send == recv is in place;
+ * reduce_loc writes root's recv only (it may be NULL elsewhere).  Buffers outside the b200mpi_alloc
+ * heap are staged whole through it (B200MPI_ERR_NOMEM if too big). */
+int b200mpi_allreduce_loc(const void* send, void* recv, size_t count, int dtype, int op, int memkind);
+int b200mpi_reduce_loc(const void* send, void* recv, size_t count, int dtype, int op, int root, int memkind);
 int b200mpi_barrier(void);
 
 /* Enqueue-only forms on the library stream (DEVICE memkind only). */

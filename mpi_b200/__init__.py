@@ -3,13 +3,15 @@
 `import mpi_b200 as mpi` gives the reference's package surface (mpi.go) over libb200mpi.so:
 Init, Finalize, Rank, Size, Send, Receive (+ Recv, Bcast, Allreduce, Allgather, Barrier,
 ReduceScatter, Reduce, Alltoall, Gather, Scatter, Gatherv, Scatterv, Allgatherv, Alltoallv,
-Scan, Exscan, ReduceScatterv, Isend/Wait).
+Scan, Exscan, ReduceScatterv, AllreduceLoc, ReduceLoc (MAXLOC / MINLOC over the LOC_F32, LOC_F64
+and LOC_I64 pair dtypes), Isend/Wait).
 The shared library (mpi_b200/lib/libb200mpi.so, built by mpi_b200/csrc/Makefile) is loaded on
 first use; nothing here computes or moves payload bytes in Python.
 """
 from ._lib import LIB_PATH, load  # noqa: F401
 from .api import (  # noqa: F401
-    MAX, MIN, SUM, Alloc, Allgather, Allgatherv, Allreduce, Alltoall, Alltoallv, Barrier, Bcast, Cuda, DeviceSlice, Exscan,
-    Finalize, Gather, Gatherv, Init, Interface, Isend, MpiError, Rank, Raw, Receive, Recv, Reduce, ReduceScatter,
-    ReduceScatterv, Register, Scan, Scatter, Scatterv, Send, Size, TagExists, Wait)
+    LOC_F32, LOC_F64, LOC_I64, MAX, MIN, SUM, Alloc, Allgather, Allgatherv, Allreduce, AllreduceLoc, Alltoall, Alltoallv,
+    Barrier, Bcast, Cuda, DeviceSlice, Exscan, Finalize, Gather, Gatherv, Init, Interface, Isend, MpiError, Rank, Raw,
+    Receive, Recv, Reduce, ReduceLoc, ReduceScatter, ReduceScatterv, Register, Scan, Scatter, Scatterv, Send, Size,
+    TagExists, Wait)
 from . import flags  # noqa: F401

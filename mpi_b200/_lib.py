@@ -56,6 +56,8 @@ SYMBOLS = {
     "b200mpi_scan": (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_size_t, _c.c_int, _c.c_int, _c.c_int]),
     "b200mpi_exscan": (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_size_t, _c.c_int, _c.c_int, _c.c_int]),
     "b200mpi_reduce_scatterv": (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.POINTER(_c.c_size_t), _c.c_int, _c.c_int, _c.c_int]),
+    "b200mpi_allreduce_loc": (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_size_t, _c.c_int, _c.c_int, _c.c_int]),
+    "b200mpi_reduce_loc": (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_size_t, _c.c_int, _c.c_int, _c.c_int, _c.c_int]),
     "b200mpi_reduce_scatter_async": (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_size_t, _c.c_int, _c.c_int]),
     "b200mpi_numa_node": (_c.c_int, []),
     "b200mpi_barrier": (_c.c_int, []),

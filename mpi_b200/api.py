@@ -11,6 +11,7 @@ Same names, same argument meaning, same blocking behaviour:
     Gatherv(send, recv, root, counts)  Scatterv(send, recv, counts, root)  Allgatherv(send, recv, counts)
     Alltoallv(send, send_counts, recv, recv_counts)                                          (new)
     ReduceScatterv(send, recv, counts, op)                                                   (new)
+    AllreduceLoc(send, recv, op)  ReduceLoc(send, recv, op, root)   (MAXLOC / MINLOC, new)
     Isend(data, destination, tag) + Wait(destination, tag)     (the Send/Wait design commented out
                                                                 in the reference, mpi.go:132-152)
 
@@ -54,6 +55,13 @@ class Raw(bytes):
 _NP2DT = {np.dtype(np.uint8): L.U8, np.dtype(np.int64): L.I64, np.dtype(np.float32): L.F32, np.dtype(np.float64): L.F64}
 _DT2NP = {v: k for k, v in _NP2DT.items()}
 
+# The value-location pairs of AllreduceLoc / ReduceLoc: the C struct {V val; int64_t loc}, 16 bytes
+# for every V (4 padding bytes after an f32 value).  Only those two calls take them.
+LOC_F32 = np.dtype([("val", "<f4"), ("loc", "<i8")], align=True)
+LOC_F64 = np.dtype([("val", "<f8"), ("loc", "<i8")], align=True)
+LOC_I64 = np.dtype([("val", "<i8"), ("loc", "<i8")], align=True)
+_LOC2DT = {LOC_F32: L.F32, LOC_F64: L.F64, LOC_I64: L.I64}
+
 
 def _check(rc, tag=None):
     if rc == 0:
@@ -69,7 +77,7 @@ class DeviceSlice:
 
     def __init__(self, count, dtype, ptr=None, owner=True):
         self.dtype = np.dtype(dtype)
-        if self.dtype not in _NP2DT:
+        if self.dtype not in _NP2DT and self.dtype not in _LOC2DT:
             raise TypeError("unsupported element type %s" % self.dtype)
         self.count = int(count)
         self._owner = owner
@@ -121,6 +129,8 @@ def Alloc(count, dtype):
 def _describe(data):
     """-> (pointer, count, dtype code, memkind, keepalive, kind tag)."""
     if isinstance(data, DeviceSlice):
+        if data.dtype not in _NP2DT:
+            raise TypeError("mpi: value-location pairs (%s) go through AllreduceLoc and ReduceLoc only" % data.dtype)
         return data.ptr, data.count, _NP2DT[data.dtype], L.DEVICE, data, "device"
     if isinstance(data, np.ndarray):
         if data.dtype not in _NP2DT:
@@ -222,7 +232,8 @@ class Cuda(Interface):
         lib = L.load()
         n = ctypes.c_size_t(0)
         if isinstance(data, DeviceSlice):
-            _check(lib.b200mpi_recv(data.ptr, data.count, ctypes.byref(n), _NP2DT[data.dtype], int(source), int(tag), L.DEVICE), tag)
+            _, _, dt, _, _, _ = _describe(data)
+            _check(lib.b200mpi_recv(data.ptr, data.count, ctypes.byref(n), dt, int(source), int(tag), L.DEVICE), tag)
             return data[: n.value]
         want_str = data is str or isinstance(data, str)
         want_bytes = data is bytes or isinstance(data, bytes)
@@ -497,6 +508,43 @@ class Cuda(Interface):
         _check(L.load().b200mpi_reduce_scatterv(sp, rp, table, sdt, int(op), sk))
         return recv, counts
 
+    @staticmethod
+    def _describe_loc(data, what):
+        """-> (pointer, count, value dtype code, memkind) of a pair array or DeviceSlice."""
+        if isinstance(data, DeviceSlice):
+            dt, ptr, kind = data.dtype, data.ptr, L.DEVICE
+        elif isinstance(data, np.ndarray):
+            if not data.flags["C_CONTIGUOUS"]:
+                raise ValueError("mpi: array must be contiguous")
+            dt, ptr, kind = data.dtype, (data.ctypes.data if data.size else None), L.HOST
+        else:
+            raise TypeError("mpi: %s takes a numpy array or DeviceSlice of pairs, not a %s" % (what, type(data).__name__))
+        if dt not in _LOC2DT:
+            raise TypeError("mpi: %s needs value-location pairs (LOC_F32, LOC_F64 or LOC_I64), not %s" % (what, dt))
+        return ptr, len(data), _LOC2DT[dt], kind
+
+    def AllreduceLoc(self, send, recv, op=MAX):
+        """MAXLOC (op MAX) / MINLOC (op MIN) over {val, loc} pairs, combined in rank order: a higher
+        rank's pair wins when its value is better, or equal with a smaller loc; NaN beats every number
+        under both ops.  Every rank's recv gets the winning pairs whole.  recv is send: in place."""
+        sp, sc, sdt, sk = self._describe_loc(send, "AllreduceLoc")
+        rp, rc_, rdt, rk = self._describe_loc(recv, "AllreduceLoc")
+        if sc != rc_ or sdt != rdt or sk != rk:
+            raise ValueError("mpi: AllreduceLoc send and recv must have the same length, pair type and memory kind")
+        _check(L.load().b200mpi_allreduce_loc(sp, rp, sc, sdt, int(op), sk))
+        return recv
+
+    def ReduceLoc(self, send, recv, op=MAX, root=0):
+        """AllreduceLoc whose result lands in root's recv only; recv may be None elsewhere."""
+        sp, sc, sdt, sk = self._describe_loc(send, "ReduceLoc")
+        rp = None
+        if recv is not None:
+            rp, rc_, rdt, rk = self._describe_loc(recv, "ReduceLoc")
+            if sc != rc_ or sdt != rdt or sk != rk:
+                raise ValueError("mpi: ReduceLoc send and recv must have the same length, pair type and memory kind")
+        _check(L.load().b200mpi_reduce_loc(sp, rp, sc, sdt, int(op), int(root), sk))
+        return recv
+
 
 # ---- package-level facade: mpi.go:56-159 -------------------------------------------------------
 _mpier = Cuda()
@@ -614,6 +662,14 @@ def Alltoallv(send, send_counts, recv=None, recv_counts=None):
 
 def ReduceScatterv(send, recv=None, counts=None, op=SUM):
     return _collective("ReduceScatterv")(send, recv, counts, op)
+
+
+def AllreduceLoc(send, recv, op=MAX):
+    return _collective("AllreduceLoc")(send, recv, op)
+
+
+def ReduceLoc(send, recv, op=MAX, root=0):
+    return _collective("ReduceLoc")(send, recv, op, root)
 
 
 def Isend(data, destination, tag):

@@ -14,7 +14,8 @@
 //   mpi.Register(impl)                         void mpi::Register(Interface*)  (second call throws = panics, mpi.go:61-67)
 //   flag.Parse() + mpi.Flag*                   mpi::ParseFlags(argc, argv) + mpi::Flag*
 //   new: Recv, Bcast, Allreduce, Allgather, Barrier, ReduceScatter, Reduce, Alltoall, Isend/Wait,
-//        Gather, Scatter, Gatherv, Scatterv, Allgatherv, Alltoallv, Scan, Exscan, ReduceScatterv;
+//        Gather, Scatter, Gatherv, Scatterv, Allgatherv, Alltoallv, Scan, Exscan, ReduceScatterv,
+//        AllreduceLoc, ReduceLoc (MAXLOC / MINLOC over mpi::ValLoc<V> pairs);
 //        mpi::DeviceSlice<T> for heap-resident buffers
 // `data` may be std::vector<double|float|int64_t|uint8_t>, std::string (sent as bytes, the
 // "anything else is gob-encoded" path), or DeviceSlice<T>.
@@ -59,6 +60,14 @@ template <> struct dtype_of<int64_t> { static constexpr int value = B200MPI_I64;
 template <> struct dtype_of<long long> { static constexpr int value = B200MPI_I64; };
 template <> struct dtype_of<float> { static constexpr int value = B200MPI_F32; };
 template <> struct dtype_of<double> { static constexpr int value = B200MPI_F64; };
+
+// The element of AllreduceLoc / ReduceLoc (MPI's MAXLOC / MINLOC pairs): 16 bytes for V = float,
+// double and int64_t.  It has no dtype_of, so no other call takes it.
+template <typename V> struct ValLoc {
+  V val;
+  int64_t loc;
+};
+static_assert(sizeof(ValLoc<float>) == 16 && sizeof(ValLoc<double>) == 16 && sizeof(ValLoc<int64_t>) == 16, "pair layout");
 
 // Memory from the rank's peer-mapped device heap: collectives and Send/Receive use it in place.
 template <typename T>
@@ -188,6 +197,9 @@ struct Interface {
   virtual Error Alltoallv(Buffer, const size_t*, Buffer, const size_t*) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Alltoallv"; return e; }
   // counts[Size()] is the same table on every rank: rank j receives the reduction of block j
   virtual Error ReduceScatterv(Buffer, Buffer, const size_t*, Op) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no ReduceScatterv"; return e; }
+  // MAXLOC (MAX) / MINLOC (MIN) over ValLoc pairs, whose value type is the Buffer's dtype
+  virtual Error AllreduceLoc(Buffer, Buffer, Op) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no AllreduceLoc"; return e; }
+  virtual Error ReduceLoc(Buffer, Buffer, Op, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no ReduceLoc"; return e; }
   // the Send/Wait pair the reference sketches and comments out (mpi.go:132-152)
   virtual Error Isend(Buffer, int, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Isend"; return e; }
   virtual Error Wait(int, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Wait"; return e; }
@@ -231,6 +243,8 @@ struct Cuda : Interface {
   Error Allgatherv(Buffer s, Buffer r, const size_t* counts) override { return make_error(b200mpi_allgatherv(s.ptr, r.ptr, counts, s.dtype, s.memkind)); }
   Error Alltoallv(Buffer s, const size_t* sc, Buffer r, const size_t* rc) override { return make_error(b200mpi_alltoallv(s.ptr, sc, r.ptr, rc, s.dtype, s.memkind)); }
   Error ReduceScatterv(Buffer s, Buffer r, const size_t* counts, Op op) override { return make_error(b200mpi_reduce_scatterv(s.ptr, r.ptr, counts, s.dtype, op, s.memkind)); }
+  Error AllreduceLoc(Buffer s, Buffer r, Op op) override { return make_error(b200mpi_allreduce_loc(s.ptr, r.ptr, s.count, s.dtype, op, s.memkind)); }
+  Error ReduceLoc(Buffer s, Buffer r, Op op, int root) override { return make_error(b200mpi_reduce_loc(s.ptr, r.ptr, s.count, s.dtype, op, root, s.memkind)); }
   Error Isend(Buffer d, int destination, int tag) override { return make_error(b200mpi_isend(d.ptr, d.count, d.dtype, destination, tag, d.memkind)); }
   Error Wait(int destination, int tag) override { return make_error(b200mpi_wait(destination, tag)); }
 };
@@ -251,6 +265,9 @@ inline void Register(Interface* impl) { // mpi.go:61-67
 template <typename T> inline Buffer lower(const std::vector<T>& v) { return {const_cast<T*>(v.data()), v.size(), dtype_of<T>::value, B200MPI_HOST}; }
 inline Buffer lower(const std::string& s) { return {const_cast<char*>(s.data()), s.size(), B200MPI_U8, B200MPI_HOST}; }
 template <typename T> inline Buffer lower(const DeviceSlice<T>& d) { return {d.data(), d.size(), dtype_of<T>::value, B200MPI_DEVICE}; }
+// pairs: count in pairs, dtype of the value
+template <typename V> inline Buffer lower_loc(const std::vector<ValLoc<V>>& v) { return {const_cast<ValLoc<V>*>(v.data()), v.size(), dtype_of<V>::value, B200MPI_HOST}; }
+template <typename V> inline Buffer lower_loc(const DeviceSlice<ValLoc<V>>& d) { return {d.data(), d.size(), dtype_of<V>::value, B200MPI_DEVICE}; }
 
 // ---- the package functions (mpi.go:96-159) -----------------------------------------------------------
 inline Error Init() { return mpier()->Init(); }
@@ -415,6 +432,24 @@ template <typename T> inline Error ReduceScatterv(const std::vector<T>& send, st
 }
 template <typename T> inline Error ReduceScatterv(const DeviceSlice<T>& send, DeviceSlice<T>* recv, const std::vector<size_t>& counts, Op op = SUM) {
   return mpier()->ReduceScatterv(lower(send), lower(*recv), counts.data(), op);
+}
+
+// AllreduceLoc: every rank's recv gets, pair by pair, the winner of MAXLOC (op MAX) or MINLOC (op
+// MIN) in rank order: a better value, or an equal one with a smaller loc; NaN beats every number.
+// ReduceLoc: root's recv only.  A vector recv is resized to len(send) (on root for ReduceLoc).
+template <typename V> inline Error AllreduceLoc(const std::vector<ValLoc<V>>& send, std::vector<ValLoc<V>>* recv, Op op = MAX) {
+  recv->resize(send.size());
+  return mpier()->AllreduceLoc(lower_loc(send), lower_loc(*recv), op);
+}
+template <typename V> inline Error AllreduceLoc(const DeviceSlice<ValLoc<V>>& send, DeviceSlice<ValLoc<V>>* recv, Op op = MAX) {
+  return mpier()->AllreduceLoc(lower_loc(send), lower_loc(*recv), op);
+}
+template <typename V> inline Error ReduceLoc(const std::vector<ValLoc<V>>& send, std::vector<ValLoc<V>>* recv, Op op, int root) {
+  if (Rank() == root) recv->resize(send.size());
+  return mpier()->ReduceLoc(lower_loc(send), lower_loc(*recv), op, root);
+}
+template <typename V> inline Error ReduceLoc(const DeviceSlice<ValLoc<V>>& send, DeviceSlice<ValLoc<V>>* recv, Op op, int root) {
+  return mpier()->ReduceLoc(lower_loc(send), lower_loc(*recv), op, root);
 }
 
 template <typename D> inline Error Isend(const D& data, int destination, int tag) { return mpier()->Isend(lower(data), destination, tag); }

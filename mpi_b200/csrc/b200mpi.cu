@@ -326,7 +326,8 @@ static int check_status() {
 // 7 gather(v), 8 scatter(v), 9 allgatherv (these three carry a hash of the counts table in `total`),
 // 10 alltoallv (whose ranks hold different tables: each adds its table digest to the signature it
 // announces, see sync_start_pairs in kernels.cuh), 11 scan, 12 exscan, 13 reduce_scatterv (which
-// carries the table hash in `total`, as 7-9 do).
+// carries the table hash in `total`, as 7-9 do), 14 allreduce_loc and reduce_loc (extra = op |
+// (root + 1) << 4, root -1 for allreduce_loc).  15 is free.
 // `total` is the element count of the whole user call when the launch is one chunk of a pipelined
 // host-slice call (ranks that disagree about the total then disagree from the first chunk on).
 static uint64_t make_sig(int coll, int dtype, int extra, int algo, size_t count, size_t total = 0) {
@@ -643,6 +644,47 @@ static int launch_scan(bool exclusive, int dtype, int op, uint64_t so, uint64_t 
         });
       },
       [&] { return fail(B200MPI_ERR_UNSUPPORTED, "scan: unsupported dtype/op (need f32, f64 or i64 with sum/max/min)"); });
+}
+
+// The value-location reductions the two-shot body is instantiated for: {f32, f64, i64} pairs with
+// MAXLOC (op MAX) and MINLOC (op MIN).  Returns f(Loc<V>{}, Op{}), or otherwise() for any other pair.
+template <typename F, typename G>
+static auto with_loc_reduction(int dtype, int op, F&& f, G&& otherwise) {
+  auto by_op = [&](auto v) {
+    using P = Loc<decltype(v)>;
+    switch (op) {
+      case B200MPI_MAX: return f(P{}, OpMaxLoc{});
+      case B200MPI_MIN: return f(P{}, OpMinLoc{});
+    }
+    return otherwise();
+  };
+  switch (dtype) {
+    case B200MPI_F32: return by_op(float{});
+    case B200MPI_F64: return by_op(double{});
+    case B200MPI_I64: return by_op((long long)0);
+  }
+  return otherwise();
+}
+
+// AllreduceLoc (root < 0) and ReduceLoc: one algorithm, the two-shot Allreduce kernel over 16-byte
+// pairs (one pair per vector) with its grid and (NR, UNROLL).  Signature code 14 carries op, root + 1,
+// dtype and count, so a rank calling Allreduce, the other of the two, or another op, dtype, count or
+// root ends the call as B200MPI_ERR_PEER on every rank.
+static int launch_allreduce_loc(int dtype, int op, uint64_t so, uint64_t ro, size_t count, int root, cudaStream_t s) {
+  const uint64_t sig = make_sig(14, dtype, op | (root + 1) << 4, 0, count);
+  return with_loc_reduction(
+      dtype, op,
+      [&](auto t, auto o) {
+        using T = decltype(t);
+        using Op = decltype(o);
+        const int n = g->ctrl.n;
+        const size_t per = (count + n - 1) / n;
+        const uint32_t sh = own_shift(count, n, 0);
+        return with_owner_tiling<T>(n, [&](auto nr, auto unroll) {
+          return launch_coll(allreduce_twoshot_kernel<T, Op, nr, unroll>, "allreduce_twoshot_kernel", sig, grid_for(per, unroll), kThreads, 0, s, so, ro, count, sh, root);
+        });
+      },
+      [] { return fail(B200MPI_ERR_UNSUPPORTED, "allreduce_loc: unsupported dtype/op (need f32, f64 or i64 pairs with max/min)"); });
 }
 
 // AUTO for Allreduce: best busbw / latency per (n, size) among the variants.  The multi-GPU thresholds
@@ -1278,6 +1320,26 @@ static int do_scan(const void* send, void* recv, size_t count, int dtype, int op
   Staging st;
   if ((rc = stage(st, memkind, send, bytes, recv, bytes, !gets ? kSendOnly : recv == send ? kRecvInSend : kApart))) return rc;
   if ((rc = launch_scan(exclusive, dtype, op, st.in, st.out, count, g->stream))) return rc;
+  return finish(false, st);
+}
+
+// MAXLOC / MINLOC over `count` 16-byte {value, int64 loc} pairs whose value type is `dtype`: into
+// every rank's recv (all) or into root's only, where recv may be NULL elsewhere.  One algorithm, no
+// host pipelining: host slices and foreign device pointers are staged whole.
+static int do_allreduce_loc(const void* send, void* recv, size_t count, int dtype, int op, int root, int memkind, bool all) {
+  const char* what = all ? "allreduce_loc" : "reduce_loc";
+  size_t es;
+  int rc = check_coll(what, all ? kReduces : kReduces | kRooted, dtype, op, root, memkind, es);
+  if (rc) return rc;
+  if (op == B200MPI_SUM) return fail(B200MPI_ERR_UNSUPPORTED, std::string(what) + ": op must be max (MAXLOC) or min (MINLOC)");
+  const bool gets = all || g->ctrl.rank == root; // this rank's recv is written
+  if (count && (!send || (gets && !recv))) return null_buffer(what);
+  if (((uintptr_t)send | (gets ? (uintptr_t)recv : 0)) & 7) return fail(B200MPI_ERR_ARG, std::string(what) + ": pair buffers must be 8-byte aligned");
+  const size_t bytes = count * sizeof(Loc<double>);
+  if (g->ctrl.n == 1) return local_copy(recv, send, bytes, memkind, false);
+  Staging st;
+  if ((rc = stage(st, memkind, send, bytes, recv, bytes, !gets ? kSendOnly : recv == send ? kRecvInSend : kApart))) return rc;
+  if ((rc = launch_allreduce_loc(dtype, op, st.in, st.out, count, all ? -1 : root, g->stream))) return rc;
   return finish(false, st);
 }
 
@@ -2200,6 +2262,12 @@ int b200mpi_reduce(const void* send, void* recv, size_t count, int dtype, int op
 int b200mpi_alltoall(const void* send, void* recv, size_t count_per_rank, int dtype, int memkind) { return do_alltoall(send, recv, count_per_rank, dtype, memkind, false); }
 int b200mpi_scan(const void* send, void* recv, size_t count, int dtype, int op, int memkind) { return do_scan(send, recv, count, dtype, op, memkind, false); }
 int b200mpi_exscan(const void* send, void* recv, size_t count, int dtype, int op, int memkind) { return do_scan(send, recv, count, dtype, op, memkind, true); }
+int b200mpi_allreduce_loc(const void* send, void* recv, size_t count, int dtype, int op, int memkind) {
+  return do_allreduce_loc(send, recv, count, dtype, op, 0, memkind, true);
+}
+int b200mpi_reduce_loc(const void* send, void* recv, size_t count, int dtype, int op, int root, int memkind) {
+  return do_allreduce_loc(send, recv, count, dtype, op, root, memkind, false);
+}
 int b200mpi_gather(const void* send, void* recv, size_t count_per_rank, int dtype, int root, int memkind) { return do_gather(send, recv, count_per_rank, dtype, root, memkind, false); }
 int b200mpi_scatter(const void* send, void* recv, size_t count_per_rank, int dtype, int root, int memkind) { return do_gather(send, recv, count_per_rank, dtype, root, memkind, true); }
 int b200mpi_gatherv(const void* send, void* recv, const size_t* counts, int dtype, int root, int memkind) { return do_gatherv(send, recv, counts, dtype, root, false, memkind); }

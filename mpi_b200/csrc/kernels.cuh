@@ -22,6 +22,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
 #include <type_traits>
 
 namespace b200 {
@@ -415,6 +416,40 @@ struct OpMin {
   template <typename T> __device__ __forceinline__ static T apply(T a, T b) { return b < a ? b : a; }
 };
 
+// A value-location pair of MAXLOC / MINLOC: the C struct { V val; int64_t loc; }, 16 bytes for f32,
+// f64 and i64 alike (4 padding bytes follow an f32 value).  `w` holds the value's bytes and the
+// padding, so that a pair is always moved whole: the winner's value bits, loc and padding.
+template <typename V>
+struct Loc {
+  unsigned long long w;
+  long long loc;
+  __host__ __device__ __forceinline__ V val() const {
+    V v;
+    memcpy(&v, &w, sizeof(V));
+    return v;
+  }
+};
+static_assert(sizeof(Loc<float>) == 16 && sizeof(Loc<double>) == 16 && sizeof(Loc<long long>) == 16, "pair size");
+
+// MAXLOC (MAX) / MINLOC (!MAX) of a (the lower ranks) and b (a higher rank): b wins when its value is
+// better, or equal with a smaller loc; on a tie of both a is kept.  Floats compare as IEEE (-0 == +0),
+// except that a NaN is better than every number under both ops and equal to every other NaN.  The
+// winner is the lowest-ranked pair among the best ones, so any bracketing of the fold agrees.
+template <bool MAX, typename V>
+__host__ __device__ __forceinline__ Loc<V> apply_loc(const Loc<V>& a, const Loc<V>& b) {
+  const V x = a.val(), y = b.val();
+  const bool xnan = x != x, ynan = y != y;
+  const bool better = xnan ? false : ynan ? true : MAX ? y > x : y < x;
+  const bool equal = xnan ? ynan : !ynan && x == y;
+  return (better || (equal && b.loc < a.loc)) ? b : a;
+}
+struct OpMaxLoc {
+  template <typename T> __host__ __device__ __forceinline__ static T apply(T a, T b) { return apply_loc<true>(a, b); }
+};
+struct OpMinLoc {
+  template <typename T> __host__ __device__ __forceinline__ static T apply(T a, T b) { return apply_loc<false>(a, b); }
+};
+
 template <typename T, typename Op>
 __device__ __forceinline__ Pack<T> combine(const Pack<T>& a, const Pack<T>& b) {
   Pack<T> r;
@@ -429,12 +464,35 @@ __device__ __forceinline__ bool all_aligned16(const uint64_t* s_a, const uint64_
   return (m & 15) == 0;
 }
 
+// Element e of the buffer at byte address p, loaded and stored through volatile accesses of the
+// element's own width.  A pair has no volatile copy: it moves as two 8-byte halves.
+template <typename T>
+struct Elem {
+  template <typename P> __device__ __forceinline__ static T ld(P p, size_t e) { return reinterpret_cast<const volatile T*>(p)[e]; }
+  template <typename P> __device__ __forceinline__ static void st(P p, size_t e, T v) { reinterpret_cast<volatile T*>(p)[e] = v; }
+};
+template <typename V>
+struct Elem<Loc<V>> {
+  template <typename P> __device__ __forceinline__ static Loc<V> ld(P p, size_t e) {
+    const volatile unsigned long long* q = reinterpret_cast<const volatile unsigned long long*>(p) + 2 * e;
+    Loc<V> x;
+    x.w = q[0];
+    x.loc = (long long)q[1];
+    return x;
+  }
+  template <typename P> __device__ __forceinline__ static void st(P p, size_t e, Loc<V> v) {
+    volatile unsigned long long* q = reinterpret_cast<volatile unsigned long long*>(p) + 2 * e;
+    q[0] = v.w;
+    q[1] = (unsigned long long)v.loc;
+  }
+};
+
 // Element e of the n buffers at byte addresses src(0), ..., src(n-1), reduced in rank order:
 // acc = x_0; acc = op(acc, x_r) for r = 1..n-1.
 template <typename T, typename Op, typename Src>
 __device__ __forceinline__ T reduce_ranks(Src src, int n, size_t e) {
-  T acc = reinterpret_cast<const volatile T*>(src(0))[e];
-  for (int r = 1; r < n; ++r) acc = Op::template apply<T>(acc, reinterpret_cast<const volatile T*>(src(r))[e]);
+  T acc = Elem<T>::ld(src(0), e);
+  for (int r = 1; r < n; ++r) acc = Op::template apply<T>(acc, Elem<T>::ld(src(r), e));
   return acc;
 }
 // ... of the n sends of a call (rank r's at heap offset s_a[r])
@@ -452,7 +510,7 @@ __device__ __forceinline__ void reduce_store_elements(const Comm& c, const uint6
   for (size_t e = lo + gtid; e < hi; e += (size_t)nb * blockDim.x) {
     const T acc = reduce_ranks<T, Op>(c, s_a, n, e);
     for (int r = 0; r < n; ++r)
-      if (only_dst < 0 || r == only_dst) reinterpret_cast<volatile T*>(c.base[r] + s_b[r])[e] = acc;
+      if (only_dst < 0 || r == only_dst) Elem<T>::st(c.base[r] + s_b[r], e, acc);
   }
 }
 

@@ -415,6 +415,58 @@ def main():
             send.free()
             recv.free()
 
+    if "allreduce_loc" in colls:
+        # MAXLOC / MINLOC, one algorithm (the two-shot body over 16-byte pairs).  Two numbers:
+        # - the blocking-call latency of one pair (median of 200 calls, max over ranks) next to a 16-byte
+        #   Allreduce under AUTO (the LL path) and under forced one-shot: whether pairs need a latency path;
+        # - 64 MiB of pairs per rank as a share of the two-shot link bound 2(n-1)/n*S at 450 GB/s per
+        #   direction (H100 SXM data sheet), time = events around back-to-back blocking calls.
+        # x_r = (r, loc r): MAXLOC ends on (n-1, n-1) everywhere.
+        if n < 2 or L.get_param("shared_device"):
+            emit({"coll": "allreduce_loc", "ok": True, "note": "fewer than two NVLink-connected GPUs (ranks %s): AllreduceLoc not measured"
+                  % ("share one GPU" if n > 1 else "= 1")})
+        else:
+            big = (64 << 20) // 16
+            pairs = np.zeros(big, dtype=mpi.LOC_F64)
+            pairs["val"], pairs["loc"] = rank, rank
+            send = mpi.Alloc(big, mpi.LOC_F64).copy_from_host(pairs)
+            recv = mpi.Alloc(big, mpi.LOC_F64)
+            plain = mpi.Alloc(4, np.float32).copy_from_host(np.full(4, rank + 1, dtype=np.float32))
+            plain_out = mpi.Alloc(4, np.float32)
+
+            def median_call(call):
+                ts = []
+                for i in range(220):
+                    mpi.Barrier() if i % 50 == 0 else None
+                    t0 = time.perf_counter()
+                    if call():
+                        raise RuntimeError(L.last_error())
+                    ts.append(time.perf_counter() - t0)
+                return maxr(sorted(ts[20:])[100])
+            row = {"coll": "allreduce_loc", "dtype": "f64", "algo": "twoshot", "bytes": 16,
+                   "t_call_us_median": median_call(lambda: lib.b200mpi_allreduce_loc(send.ptr, recv.ptr, 1, L.F64, L.MAX, L.DEVICE)) * 1e6}
+            for algo in ("auto", "oneshot"):
+                lib.b200mpi_set_algo(L.COLL_ALLREDUCE, ALGOS[algo])
+                row["allreduce_16B_%s_t_call_us_median" % algo] = median_call(
+                    lambda: lib.b200mpi_allreduce(plain.ptr, plain_out.ptr, 4, L.F32, L.MAX, L.DEVICE)) * 1e6
+            lib.b200mpi_set_algo(L.COLL_ALLREDUCE, 0)
+            row["ok"] = maxr(0.0 if recv[:1].to_host()["loc"][0] == n - 1 else 1.0) == 0.0
+            emit(row)
+            S = big * 16
+
+            def blocking():
+                if lib.b200mpi_allreduce_loc(send.ptr, recv.ptr, big, L.F64, L.MAX, L.DEVICE):
+                    raise RuntimeError(L.last_error())
+            it, wm = iters_for(S)
+            t = timed(blocking, it, wm)
+            got = recv[:64].to_host()
+            ok = maxr(0.0 if bool(np.all(got["loc"] == n - 1) and np.all(got["val"] == n - 1)) else 1.0) == 0.0
+            bound = 2 * (n - 1) / n * S / 450e9
+            emit({"coll": "allreduce_loc", "dtype": "f64", "algo": "twoshot", "bytes": S, "t_us": t * 1e6, "algbw_gbs": S / t / 1e9,
+                  "link_bytes": 2 * (n - 1) / n * S, "link_roofline_share": bound / t, "ok": ok})
+            for b in (send, recv, plain, plain_out):
+                b.free()
+
     if "p2p" in colls and n > 1:
         # bounce (examples/bounce/bounce.go:85-138): even sends, odd returns; device-resident float64
         maxp = min(args.max_bytes, 256 << 20)

@@ -87,6 +87,19 @@ func Alloc(prototype interface{}, n int) (*DeviceSlice, error) {
 // Free returns the slice to the heap.
 func (d *DeviceSlice) Free() { C.b200mpi_free(d.Ptr); d.Ptr = nil }
 
+// elemSize is the bytes of one element (16 for a value-location pair).
+func (d *DeviceSlice) elemSize() int {
+	switch {
+	case d.loc:
+		return 16
+	case d.dtype == dtU8:
+		return 1
+	case d.dtype == dtF32:
+		return 4
+	}
+	return 8
+}
+
 func lastError(rc C.int, tag int) error {
 	msg := C.GoString(C.b200mpi_last_error())
 	if rc == C.B200MPI_ERR_TAG_EXISTS {
@@ -756,6 +769,78 @@ func (c *Cuda) ReduceLoc(send, recv interface{}, op Op, root int) error {
 		}
 	}
 	if rc := C.b200mpi_reduce_loc(sp, rp, C.size_t(sn), sdt, C.int(op), C.int(root), sk); rc != 0 {
+		return lastError(rc, 0)
+	}
+	return nil
+}
+
+// cudaWindow is a Window of libb200mpi: the id b200mpi_win_create handed out.
+type cudaWindow struct{ id C.int }
+
+// WinCreate: local's bytes (a pair slice too: a window is untyped memory), or an empty window for nil.
+func (c *Cuda) WinCreate(local *DeviceSlice) (Window, error) {
+	var base unsafe.Pointer
+	var bytes C.size_t
+	if local != nil {
+		base, bytes = local.Ptr, C.size_t(local.Len*local.elemSize())
+	}
+	var id C.int
+	if rc := C.b200mpi_win_create(base, bytes, &id); rc != 0 {
+		return nil, lastError(rc, 0)
+	}
+	return &cudaWindow{id: id}, nil
+}
+
+// lowerOrigin is lowerTyped for the one-sided calls, which also refuse a negative displacement.
+func lowerOrigin(what string, origin interface{}, disp int) (unsafe.Pointer, int, C.int, C.int, error) {
+	if disp < 0 {
+		return nil, 0, 0, 0, fmt.Errorf("mpi: %s displacement must be >= 0", what)
+	}
+	return lowerTyped(what, origin)
+}
+
+func (w *cudaWindow) Put(origin interface{}, target, disp int) error {
+	p, n, dt, mk, err := lowerOrigin("Put", origin, disp)
+	if err != nil {
+		return err
+	}
+	if rc := C.b200mpi_put(p, C.size_t(n), dt, C.int(target), C.size_t(disp), w.id, mk); rc != 0 {
+		return lastError(rc, 0)
+	}
+	return nil
+}
+
+func (w *cudaWindow) Get(origin interface{}, target, disp int) error {
+	p, n, dt, mk, err := lowerOrigin("Get", origin, disp)
+	if err != nil {
+		return err
+	}
+	if rc := C.b200mpi_get(p, C.size_t(n), dt, C.int(target), C.size_t(disp), w.id, mk); rc != 0 {
+		return lastError(rc, 0)
+	}
+	return nil
+}
+
+func (w *cudaWindow) Accumulate(origin interface{}, target, disp int, op Op) error {
+	p, n, dt, mk, err := lowerOrigin("Accumulate", origin, disp)
+	if err != nil {
+		return err
+	}
+	if rc := C.b200mpi_accumulate(p, C.size_t(n), dt, C.int(op), C.int(target), C.size_t(disp), w.id, mk); rc != 0 {
+		return lastError(rc, 0)
+	}
+	return nil
+}
+
+func (w *cudaWindow) Fence() error {
+	if rc := C.b200mpi_win_fence(w.id); rc != 0 {
+		return lastError(rc, 0)
+	}
+	return nil
+}
+
+func (w *cudaWindow) Free() error {
+	if rc := C.b200mpi_win_free(w.id); rc != 0 {
 		return lastError(rc, 0)
 	}
 	return nil

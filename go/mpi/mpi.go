@@ -30,6 +30,7 @@
 //	Scan, Exscan                      prefix reductions in rank order (inclusive, exclusive)
 //	ReduceScatterv                    ReduceScatter with a different block length for every rank
 //	AllreduceLoc, ReduceLoc           MAXLOC / MINLOC: the best value across ranks and where it came from
+//	WinCreate -> Window               one-sided Put, Get and Accumulate into other ranks' heap memory, completed by Fence
 //	Isend + Wait   the non-blocking Send design the reference sketches and comments out (mpi.go:132-152)
 //
 // They are served through the optional Collective interface, the upgrade the reference hints at
@@ -108,6 +109,29 @@ type Collective6 interface {
 type Collective7 interface {
 	AllreduceLoc(send, recv interface{}, op Op) error
 	ReduceLoc(send, recv interface{}, op Op, root int) error
+}
+
+// Collective8 is the eighth optional upgrade: one-sided communication (MPI-3 active target with
+// fence synchronisation) through windows of every rank's device heap.
+type Collective8 interface {
+	WinCreate(local *DeviceSlice) (Window, error)
+}
+
+// Window is memory of every rank's heap that any rank may Put into, Get from and Accumulate into.
+// origin is a []float64, []float32, []int64, []byte or *DeviceSlice; disp counts elements of the
+// origin's type from the start of rank target's window, and the range must fit in it. Each call
+// returns once origin may be reused (Get: once it holds the data). What Put and Accumulate write is
+// visible to the target after its next Fence, which every rank calls; a location written by one
+// rank and read or written by another between two fences is undefined, except by Accumulates with
+// the same type and op. Accumulate (Sum, Max, Min over float32, float64 and int64) is element-wise
+// atomic: int64 Sum wraps, float32 Sum flushes subnormal values to zero, float Max and Min keep a NaN
+// already in the target and ignore a NaN in origin. Free is a Fence that also drops the window.
+type Window interface {
+	Put(origin interface{}, target, disp int) error
+	Get(origin interface{}, target, disp int) error
+	Accumulate(origin interface{}, target, disp int, op Op) error
+	Fence() error
+	Free() error
 }
 
 // Float32Loc, Float64Loc and Int64Loc are the elements of AllreduceLoc and ReduceLoc: a value and
@@ -429,4 +453,14 @@ func ReduceLoc(send, recv interface{}, op Op, root int) error {
 		return err
 	}
 	return c.ReduceLoc(send, recv, op, root)
+}
+
+// WinCreate is collective: every rank exposes local, a *DeviceSlice from Alloc (nil for an empty
+// window), to one-sided calls by every rank. Windows may differ in size from rank to rank.
+func WinCreate(local *DeviceSlice) (Window, error) {
+	c, ok := current.(Collective8)
+	if !ok {
+		return nil, fmt.Errorf("mpi: registered implementation %T has no WinCreate", current)
+	}
+	return c.WinCreate(local)
 }

@@ -32,7 +32,8 @@ extern "C" {
 
 #define B200MPI_VERSION 200 /* 0.2.0: + isend/wait, reduce_scatter, reduce, alltoall, probes, get_param;
                                then gather, scatter, gatherv, scatterv, allgatherv, alltoallv, scan, exscan,
-                               reduce_scatterv, allreduce_loc, reduce_loc (all additive) */
+                               reduce_scatterv, allreduce_loc, reduce_loc, win_create, win_free, win_fence,
+                               put, get, accumulate (all additive) */
 #define B200MPI_MAX_RANKS 8 /* "the 8 GPUs of one box" */
 
 typedef enum {
@@ -208,6 +209,45 @@ int b200mpi_reduce_scatterv(const void* send, void* recv, const size_t* counts, 
 int b200mpi_allreduce_loc(const void* send, void* recv, size_t count, int dtype, int op, int memkind);
 int b200mpi_reduce_loc(const void* send, void* recv, size_t count, int dtype, int op, int root, int memkind);
 int b200mpi_barrier(void);
+
+/* ---- one-sided communication: windows, Put / Get / Accumulate, fence (MPI-3 active target) ------ */
+
+/* A window is [base, base + bytes) of this rank's b200mpi_alloc heap (anything else:
+ * B200MPI_ERR_ARG); sizes may differ from rank to rank, and bytes == 0 with base == NULL is legal.
+ * The library does not own the memory: freeing it while the window is live is erroneous (not
+ * checked).  win_create is collective: every rank learns every rank's window, *win gets an id
+ * handed out in call order and never reused; ranks whose ids differ, or whose peers refused their
+ * arguments, get B200MPI_ERR_PEER and no window is created.  A freed or unknown id: B200MPI_ERR_ARG.
+ * win_free is collective: a win_fence, then the id is dropped. */
+int b200mpi_win_create(void* base, size_t bytes, int* win);
+int b200mpi_win_free(int win);
+/* Collective: every Put and Accumulate any rank issued into this window before its fence is visible
+ * to the target once the target's win_fence returns, and every Get issued after a fence reads what
+ * was there at that fence.  A fence on another window, or against b200mpi_barrier, ends as
+ * B200MPI_ERR_PEER on every rank.  Within one fence epoch, a location written by one rank and read
+ * or written by another (the target's own kernels and copies included, Put against Accumulate, and
+ * Accumulates with different ops) is undefined, as in MPI. */
+int b200mpi_win_fence(int win);
+/* count elements of dtype between origin (memkind) and element target_disp of rank target's window:
+ * (target_disp + count) * element size must fit in it (B200MPI_ERR_ARG).  Blocking: each returns once
+ * origin may be reused; get's origin then holds the data.  Not collective (only the origin rank
+ * calls them, on its collective thread) and they take no barrier epoch.  count == 0 returns 0 and
+ * does nothing; a NULL origin with count > 0, a target out of range or an unknown dtype is
+ * B200MPI_ERR_ARG.  Origins outside the heap are staged whole through it (B200MPI_ERR_NOMEM if too
+ * big).  Put and Get take any alignment. */
+int b200mpi_put(const void* origin, size_t count, int dtype, int target, size_t target_disp, int win, int memkind);
+int b200mpi_get(void* origin, size_t count, int dtype, int target, size_t target_disp, int win, int memkind);
+/* target[e] = target[e] op origin[e], each element an atomic read-modify-write at system scope, so
+ * concurrent Accumulates with the same dtype and op on overlapping elements, from any ranks, combine
+ * in some order.  dtype f32, f64 or i64 (u8: B200MPI_ERR_UNSUPPORTED); op SUM, MAX or MIN (unknown:
+ * B200MPI_ERR_ARG); the target element address must be a multiple of the element size
+ * (B200MPI_ERR_ARG).  i64 SUM wraps; i64 MAX and MIN are exact; f64 SUM is one round-to-nearest add
+ * per contribution, in an unspecified order.  f32 SUM flushes subnormals: on sm_90a an f32 atomic add
+ * turns a subnormal input or result into zero of the same sign, unlike Allreduce, which keeps
+ * subnormals.  f32 and f64 MAX and MIN apply b > a ? b : a (a = the target's value), so the result
+ * does not depend on the order except for NaNs (a NaN in the target stays, a NaN contribution is
+ * dropped) and zeros of mixed sign. */
+int b200mpi_accumulate(const void* origin, size_t count, int dtype, int op, int target, size_t target_disp, int win, int memkind);
 
 /* Enqueue-only forms on the library stream (DEVICE memkind only). */
 int b200mpi_bcast_async(void* buf, size_t count, int dtype, int root);

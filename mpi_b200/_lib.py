@@ -58,6 +58,12 @@ SYMBOLS = {
     "b200mpi_reduce_scatterv": (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.POINTER(_c.c_size_t), _c.c_int, _c.c_int, _c.c_int]),
     "b200mpi_allreduce_loc": (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_size_t, _c.c_int, _c.c_int, _c.c_int]),
     "b200mpi_reduce_loc": (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_size_t, _c.c_int, _c.c_int, _c.c_int, _c.c_int]),
+    "b200mpi_win_create": (_c.c_int, [_c.c_void_p, _c.c_size_t, _c.POINTER(_c.c_int)]),
+    "b200mpi_win_free": (_c.c_int, [_c.c_int]),
+    "b200mpi_win_fence": (_c.c_int, [_c.c_int]),
+    "b200mpi_put": (_c.c_int, [_c.c_void_p, _c.c_size_t, _c.c_int, _c.c_int, _c.c_size_t, _c.c_int, _c.c_int]),
+    "b200mpi_get": (_c.c_int, [_c.c_void_p, _c.c_size_t, _c.c_int, _c.c_int, _c.c_size_t, _c.c_int, _c.c_int]),
+    "b200mpi_accumulate": (_c.c_int, [_c.c_void_p, _c.c_size_t, _c.c_int, _c.c_int, _c.c_int, _c.c_size_t, _c.c_int, _c.c_int]),
     "b200mpi_reduce_scatter_async": (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_size_t, _c.c_int, _c.c_int]),
     "b200mpi_numa_node": (_c.c_int, []),
     "b200mpi_barrier": (_c.c_int, []),

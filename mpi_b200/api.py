@@ -12,6 +12,7 @@ Same names, same argument meaning, same blocking behaviour:
     Alltoallv(send, send_counts, recv, recv_counts)                                          (new)
     ReduceScatterv(send, recv, counts, op)                                                   (new)
     AllreduceLoc(send, recv, op)  ReduceLoc(send, recv, op, root)   (MAXLOC / MINLOC, new)
+    WinCreate(local) -> Win: Put, Get, Accumulate, Fence, Free      (one-sided, fence-synchronised, new)
     Isend(data, destination, tag) + Wait(destination, tag)     (the Send/Wait design commented out
                                                                 in the reference, mpi.go:132-152)
 
@@ -546,6 +547,66 @@ class Cuda(Interface):
         return recv
 
 
+    # -- one-sided communication ----------------------------------------------------------------
+    def WinCreate(self, local):
+        """Collective: exposes `local`, a DeviceSlice from Alloc (or None for an empty window), to
+        one-sided Put, Get and Accumulate by every rank.  Windows may differ in size from rank to rank."""
+        if local is None:
+            ptr, nbytes = None, 0
+        elif isinstance(local, DeviceSlice):
+            ptr, nbytes = local.ptr, local.nbytes
+        else:
+            raise TypeError("mpi: a window is a DeviceSlice from Alloc (or None), not a %s" % type(local).__name__)
+        wid = ctypes.c_int(-1)
+        _check(L.load().b200mpi_win_create(ptr, nbytes, ctypes.byref(wid)))
+        return Win(wid.value)
+
+
+class Win:
+    """A window of every rank's heap (WinCreate).  Put, Get and Accumulate move the origin's elements
+    to or from element `disp` of rank `target`'s window, counted in the origin's element type, and
+    block until the origin may be reused (Get: until it holds the data).  What they write is visible
+    to the target after its next Fence, which every rank calls; a location written by one rank and
+    read or written by another between two fences is undefined, except by Accumulates with the same
+    type and op.  Free is a Fence that also drops the window."""
+
+    def __init__(self, wid):
+        self.id = wid
+
+    @staticmethod
+    def _origin(origin, disp, what):
+        """-> (pointer, count, dtype code, memkind); refuses pairs and negative displacements."""
+        ptr, count, dt, kind, _, _ = _describe(origin)
+        if int(disp) < 0:
+            raise ValueError("mpi: %s displacement must be >= 0" % what)
+        return ptr, count, dt, kind
+
+    def Put(self, origin, target, disp=0):
+        ptr, count, dt, kind = self._origin(origin, disp, "Put")
+        _check(L.load().b200mpi_put(ptr, count, dt, int(target), int(disp), self.id, kind))
+
+    def Get(self, origin, target, disp=0):
+        """Fills `origin` (a numpy array, bytearray or DeviceSlice) from the target's window and returns it."""
+        if (isinstance(origin, (str, bytes)) or (isinstance(origin, memoryview) and origin.readonly)
+                or (isinstance(origin, np.ndarray) and not origin.flags["WRITEABLE"])):
+            raise TypeError("mpi: Get needs a writable buffer (numpy array, bytearray or DeviceSlice)")
+        ptr, count, dt, kind = self._origin(origin, disp, "Get")
+        _check(L.load().b200mpi_get(ptr, count, dt, int(target), int(disp), self.id, kind))
+        return origin
+
+    def Accumulate(self, origin, target, disp=0, op=SUM):
+        """target[disp + i] = target[disp + i] op origin[i], element by element and atomically, for
+        float32, float64 and int64 (an f32 SUM flushes subnormals to zero; see b200mpi.h)."""
+        ptr, count, dt, kind = self._origin(origin, disp, "Accumulate")
+        _check(L.load().b200mpi_accumulate(ptr, count, dt, int(op), int(target), int(disp), self.id, kind))
+
+    def Fence(self):
+        _check(L.load().b200mpi_win_fence(self.id))
+
+    def Free(self):
+        _check(L.load().b200mpi_win_free(self.id))
+
+
 # ---- package-level facade: mpi.go:56-159 -------------------------------------------------------
 _mpier = Cuda()
 _register_called = False
@@ -670,6 +731,10 @@ def AllreduceLoc(send, recv, op=MAX):
 
 def ReduceLoc(send, recv, op=MAX, root=0):
     return _collective("ReduceLoc")(send, recv, op, root)
+
+
+def WinCreate(local):
+    return _collective("WinCreate")(local)
 
 
 def Isend(data, destination, tag):

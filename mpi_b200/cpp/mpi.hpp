@@ -15,7 +15,8 @@
 //   flag.Parse() + mpi.Flag*                   mpi::ParseFlags(argc, argv) + mpi::Flag*
 //   new: Recv, Bcast, Allreduce, Allgather, Barrier, ReduceScatter, Reduce, Alltoall, Isend/Wait,
 //        Gather, Scatter, Gatherv, Scatterv, Allgatherv, Alltoallv, Scan, Exscan, ReduceScatterv,
-//        AllreduceLoc, ReduceLoc (MAXLOC / MINLOC over mpi::ValLoc<V> pairs);
+//        AllreduceLoc, ReduceLoc (MAXLOC / MINLOC over mpi::ValLoc<V> pairs),
+//        WinCreate -> mpi::Window with Put, Get, Accumulate, Fence, Free (one-sided, fence-synchronised);
 //        mpi::DeviceSlice<T> for heap-resident buffers
 // `data` may be std::vector<double|float|int64_t|uint8_t>, std::string (sent as bytes, the
 // "anything else is gob-encoded" path), or DeviceSlice<T>.
@@ -200,6 +201,14 @@ struct Interface {
   // MAXLOC (MAX) / MINLOC (MIN) over ValLoc pairs, whose value type is the Buffer's dtype
   virtual Error AllreduceLoc(Buffer, Buffer, Op) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no AllreduceLoc"; return e; }
   virtual Error ReduceLoc(Buffer, Buffer, Op, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no ReduceLoc"; return e; }
+  // one-sided: a window of `bytes` at `base` of this rank's heap gets an id; Put / Get / Accumulate
+  // move a Buffer to or from element `disp` of rank `target`'s window
+  virtual Error WinCreate(void*, size_t, int*) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no WinCreate"; return e; }
+  virtual Error WinFree(int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no WinFree"; return e; }
+  virtual Error WinFence(int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no WinFence"; return e; }
+  virtual Error Put(Buffer, int, size_t, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Put"; return e; }
+  virtual Error Get(Buffer, int, size_t, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Get"; return e; }
+  virtual Error Accumulate(Buffer, Op, int, size_t, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Accumulate"; return e; }
   // the Send/Wait pair the reference sketches and comments out (mpi.go:132-152)
   virtual Error Isend(Buffer, int, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Isend"; return e; }
   virtual Error Wait(int, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Wait"; return e; }
@@ -245,6 +254,14 @@ struct Cuda : Interface {
   Error ReduceScatterv(Buffer s, Buffer r, const size_t* counts, Op op) override { return make_error(b200mpi_reduce_scatterv(s.ptr, r.ptr, counts, s.dtype, op, s.memkind)); }
   Error AllreduceLoc(Buffer s, Buffer r, Op op) override { return make_error(b200mpi_allreduce_loc(s.ptr, r.ptr, s.count, s.dtype, op, s.memkind)); }
   Error ReduceLoc(Buffer s, Buffer r, Op op, int root) override { return make_error(b200mpi_reduce_loc(s.ptr, r.ptr, s.count, s.dtype, op, root, s.memkind)); }
+  Error WinCreate(void* base, size_t bytes, int* win) override { return make_error(b200mpi_win_create(base, bytes, win)); }
+  Error WinFree(int win) override { return make_error(b200mpi_win_free(win)); }
+  Error WinFence(int win) override { return make_error(b200mpi_win_fence(win)); }
+  Error Put(Buffer o, int target, size_t disp, int win) override { return make_error(b200mpi_put(o.ptr, o.count, o.dtype, target, disp, win, o.memkind)); }
+  Error Get(Buffer o, int target, size_t disp, int win) override { return make_error(b200mpi_get(o.ptr, o.count, o.dtype, target, disp, win, o.memkind)); }
+  Error Accumulate(Buffer o, Op op, int target, size_t disp, int win) override {
+    return make_error(b200mpi_accumulate(o.ptr, o.count, o.dtype, op, target, disp, win, o.memkind));
+  }
   Error Isend(Buffer d, int destination, int tag) override { return make_error(b200mpi_isend(d.ptr, d.count, d.dtype, destination, tag, d.memkind)); }
   Error Wait(int destination, int tag) override { return make_error(b200mpi_wait(destination, tag)); }
 };
@@ -451,6 +468,25 @@ template <typename V> inline Error ReduceLoc(const std::vector<ValLoc<V>>& send,
 template <typename V> inline Error ReduceLoc(const DeviceSlice<ValLoc<V>>& send, DeviceSlice<ValLoc<V>>* recv, Op op, int root) {
   return mpier()->ReduceLoc(lower_loc(send), lower_loc(*recv), op, root);
 }
+
+// One-sided communication through a window of every rank's heap (WinCreate, collective).  Put, Get
+// and Accumulate move the origin (a vector or DeviceSlice) to or from element `disp` of rank
+// `target`'s window, counted in the origin's element type, and return once the origin may be reused
+// (Get: holds the data).  Their writes are visible to the target after its next Fence, which every
+// rank calls; Free is a Fence that also drops the window.  Accumulate (SUM, MAX, MIN over float,
+// double and int64_t) is element-wise atomic; an f32 SUM flushes subnormals to zero (b200mpi.h).
+class Window {
+ public:
+  int id = -1;
+  template <typename D> Error Put(const D& origin, int target, size_t disp) { return mpier()->Put(lower(origin), target, disp, id); }
+  template <typename T> Error Get(std::vector<T>* origin, int target, size_t disp) { return mpier()->Get(lower(*origin), target, disp, id); }
+  template <typename T> Error Get(DeviceSlice<T>* origin, int target, size_t disp) { return mpier()->Get(lower(*origin), target, disp, id); }
+  template <typename D> Error Accumulate(const D& origin, int target, size_t disp, Op op = SUM) { return mpier()->Accumulate(lower(origin), op, target, disp, id); }
+  Error Fence() { return mpier()->WinFence(id); }
+  Error Free() { return mpier()->WinFree(id); }
+};
+template <typename T> inline Error WinCreate(const DeviceSlice<T>& local, Window* win) { return mpier()->WinCreate(local.data(), local.size() * sizeof(T), &win->id); }
+inline Error WinCreate(std::nullptr_t, Window* win) { return mpier()->WinCreate(nullptr, 0, &win->id); } // an empty window
 
 template <typename D> inline Error Isend(const D& data, int destination, int tag) { return mpier()->Isend(lower(data), destination, tag); }
 inline Error Wait(int destination, int tag) { return mpier()->Wait(destination, tag); }

@@ -161,6 +161,14 @@ struct Ctx {
   size_t hybrid_min_bytes = 32u << 20;
   int nvls_min_ranks = 4; // below this the fused two-shot moves fewer bytes per link than NVLS
   size_t own_block_bytes = 1u << 20; // interleave granularity of slice ownership (Owner in kernels.cuh)
+  // One-sided windows (b200mpi_win_create), indexed by window id: ids are handed out in call order and
+  // never reused, so a freed window keeps its entry with live == false.  Every rank's heap offset and
+  // size of each window, learnt at creation.  Dropped with the Ctx at teardown.
+  struct Win {
+    bool live;
+    uint64_t off[B200MPI_MAX_RANKS], bytes[B200MPI_MAX_RANKS];
+  };
+  std::vector<Win> wins;
 };
 
 static_assert(kHeapReserved == kCtrlBytes, "heap.h and kernels.cuh disagree about the control region");
@@ -327,7 +335,7 @@ static int check_status() {
 // 10 alltoallv (whose ranks hold different tables: each adds its table digest to the signature it
 // announces, see sync_start_pairs in kernels.cuh), 11 scan, 12 exscan, 13 reduce_scatterv (which
 // carries the table hash in `total`, as 7-9 do), 14 allreduce_loc and reduce_loc (extra = op |
-// (root + 1) << 4, root -1 for allreduce_loc).  15 is free.
+// (root + 1) << 4, root -1 for allreduce_loc), 15 win_fence and win_free (count = the window id).
 // `total` is the element count of the whole user call when the launch is one chunk of a pipelined
 // host-slice call (ranks that disagree about the total then disagree from the first chunk on).
 static uint64_t make_sig(int coll, int dtype, int extra, int algo, size_t count, size_t total = 0) {
@@ -356,15 +364,20 @@ static int launch_coll(void (*kernel)(Comm, P...), const char* what, uint64_t si
   return launch_check(what);
 }
 
+// The grid of launch_copy (and of accumulate_kernel) for `bytes`: one 256-thread CTA per 64 KiB, up
+// to one CTA per SM (or max_blocks).
+static int copy_grid(size_t bytes) {
+  constexpr size_t kPerBlock = 256 * 16 * 16; // bytes one CTA of copy_bytes_kernel moves per grid pass
+  const size_t want = (bytes + kPerBlock - 1) / kPerBlock;
+  const size_t cap = g->max_blocks > 0 ? (size_t)g->max_blocks : (size_t)g->sm_count;
+  return (int)std::max<size_t>(1, std::min(want, cap));
+}
+
 // dst <- src on `s` with the library's own copy kernel (local HBM or peer mapping), any alignment:
 // 256 threads x 16 vectors in flight per thread, up to one CTA per SM (or max_blocks).
 static int launch_copy(void* dst, const void* src, size_t bytes, cudaStream_t s) {
   if (bytes == 0) return 0;
-  constexpr size_t kPerBlock = 256 * 16 * 16; // bytes one CTA moves per grid pass
-  const size_t want = (bytes + kPerBlock - 1) / kPerBlock;
-  const size_t cap = g->max_blocks > 0 ? (size_t)g->max_blocks : (size_t)g->sm_count;
-  const int blocks = (int)std::max<size_t>(1, std::min(want, cap));
-  copy_bytes_kernel<16, 256, 1><<<blocks, 256, 0, s>>>((unsigned char*)dst, (const unsigned char*)src, bytes);
+  copy_bytes_kernel<16, 256, 1><<<copy_grid(bytes), 256, 0, s>>>((unsigned char*)dst, (const unsigned char*)src, bytes);
   return launch_check("copy_bytes_kernel");
 }
 
@@ -1532,6 +1545,119 @@ static int do_alltoallv(const void* send, const size_t* send_counts, void* recv,
 }
 
 // ---------------------------------------------------------------------------------------------
+// One-sided communication (active target, fence synchronisation).  A window is a range of each
+// rank's heap whose offset and size every rank learns at win_create, so a Put, Get or Accumulate is
+// one kernel between the origin (or its staging block) and base[target] + offset: not a collective,
+// it takes no epoch.  Every RMA call is blocking, so at a fence this rank's RMA kernels have
+// completed; the fence is then the barrier kernel under signature code 15 with the window id, whose
+// release / acquire flags at system scope order those writes before every rank's later work.
+// ---------------------------------------------------------------------------------------------
+static Ctx::Win* find_win(int win) {
+  return win >= 0 && (size_t)win < g->wins.size() && g->wins[win].live ? &g->wins[win] : nullptr;
+}
+static int unknown_win(const char* what) { return fail(B200MPI_ERR_ARG, std::string(what) + ": unknown or freed window"); }
+
+// Collective.  Every rank announces {next id, heap offset, bytes, its own verdict on its arguments},
+// so a rank with bad arguments fails with B200MPI_ERR_ARG and the others with B200MPI_ERR_PEER, and
+// no rank creates the window.
+static int do_win_create(void* base, size_t bytes, int* win) {
+  int rc = need_data_plane();
+  if (rc) return rc;
+  size_t off = 0;
+  const char* bad = nullptr;
+  if (!win) bad = "NULL result pointer";
+  else if ((base || bytes) && (!base || bytes > g->heap.size || !g->heap.contains(base, bytes, off)))
+    bad = "window memory must lie in this rank's b200mpi_alloc heap (or be 0 bytes at NULL)";
+  struct { uint64_t id, off, bytes, bad; } mine = {g->wins.size(), off, bytes, bad ? 1u : 0u}, all[B200MPI_MAX_RANKS];
+  std::string err;
+  if ((rc = g->ctrl.allgather(&mine, sizeof mine, all, err, g->watchdog_ns > 0 ? g->watchdog_ns : -1))) return fail(rc, "win_create: " + err);
+  if (bad) return fail(B200MPI_ERR_ARG, std::string("win_create: ") + bad);
+  Ctx::Win w = {true, {}, {}};
+  for (int r = 0; r < g->ctrl.n; ++r) {
+    if (all[r].bad) return fail(B200MPI_ERR_PEER, "win_create: rank " + std::to_string(r) + " refused its arguments");
+    if (all[r].id != mine.id) return fail(B200MPI_ERR_PEER, "win_create: ranks disagree about the window id (" + std::to_string(all[r].id) + " on rank " + std::to_string(r) + ", " + std::to_string(mine.id) + " here)");
+    w.off[r] = all[r].off;
+    w.bytes[r] = all[r].bytes;
+  }
+  g->wins.push_back(w);
+  *win = (int)mine.id;
+  return 0;
+}
+
+// Collective: the barrier kernel under signature 15 carrying the window id, so a fence on another
+// window or a Barrier ends as B200MPI_ERR_PEER on every rank.  A world of one synchronises the stream.
+// free: the window is dropped once the fence has succeeded.
+static int do_win_fence(int win, bool free) {
+  const char* what = free ? "win_free" : "win_fence";
+  int rc = need_data_plane();
+  if (rc) return rc;
+  if (!find_win(win)) return unknown_win(what);
+  if (g->ctrl.n > 1 && (rc = launch_coll(barrier_kernel, "barrier_kernel", make_sig(15, 0, 0, 0, (size_t)win), 1, 32, 0, g->stream))) return rc;
+  if ((rc = finish(false))) return rc;
+  if (free) g->wins[win].live = false;
+  return 0;
+}
+
+static int launch_accumulate(int dtype, int op, void* dst, const void* src, size_t count, cudaStream_t s) {
+  return with_reduction(
+      dtype, op,
+      [&](auto t, auto o) {
+        using T = decltype(t);
+        accumulate_kernel<T, decltype(o)><<<copy_grid(count * sizeof(T)), 256, 0, s>>>((T*)dst, (const T*)src, count);
+        return launch_check("accumulate_kernel");
+      },
+      [] { return fail(B200MPI_ERR_UNSUPPORTED, "accumulate: unsupported dtype/op (need f32, f64 or i64 with sum/max/min)"); });
+}
+
+enum RmaKind { kPut, kGet, kAccumulate };
+
+// `count` elements of `dtype` between origin and element target_disp of `target`'s window.  Blocking:
+// returns once origin may be reused (Get: holds the data).  Host origins and device pointers outside
+// the heap are staged whole, through block 0 (Put, Accumulate) or block 1 (Get).
+static int do_rma(RmaKind kind, const void* origin, size_t count, int dtype, int op, int target, size_t target_disp, int win, int memkind) {
+  static const char* const names[] = {"put", "get", "accumulate"};
+  const char* what = names[kind];
+  int rc = need_data_plane();
+  if (rc) return rc;
+  auto arg = [&](const char* msg) { return fail(B200MPI_ERR_ARG, std::string(what) + ": " + msg); };
+  const Ctx::Win* w = find_win(win);
+  if (!w) return unknown_win(what);
+  const size_t es = esize(dtype);
+  if (es == 0) return arg("unknown dtype");
+  if (kind == kAccumulate && dtype == B200MPI_U8) return fail(B200MPI_ERR_UNSUPPORTED, "accumulate: dtype must be f32, f64 or i64");
+  if (kind == kAccumulate && (op < B200MPI_SUM || op > B200MPI_MIN)) return arg("unknown op");
+  if (target < 0 || target >= g->ctrl.n) return arg("target out of range");
+  if (memkind != B200MPI_HOST && memkind != B200MPI_DEVICE) return arg("bad memkind");
+  if (count == 0) return 0;
+  if (!origin) return arg("NULL origin with count > 0");
+  // (target_disp + count) * es <= window bytes, without overflow
+  if (target_disp > SIZE_MAX - count || target_disp + count > w->bytes[target] / es) return arg("target_disp + count elements exceed the target's window");
+  const uint64_t at = w->off[target] + target_disp * es; // in the target's heap
+  if (kind == kAccumulate && at % es) return arg("target element address is not a multiple of the element size");
+  const size_t bytes = count * es;
+  char* const remote = (char*)g->heap.base[target] + at;
+  char* const local = (char*)g->heap.base[g->ctrl.rank];
+  Buf b;
+  if (kind == kGet) {
+    if ((rc = resolve(origin, bytes, memkind, 1, false, b))) return rc;
+    if ((rc = launch_copy(local + b.off, remote, bytes, g->stream))) return rc;
+    return finish(false, Staging{0, b.off, b.staged ? const_cast<void*>(origin) : nullptr, bytes, memkind});
+  }
+  if ((rc = resolve(origin, bytes, memkind, 0, true, b))) return rc;
+  if (kind == kPut) {
+    rc = launch_copy(remote, local + b.off, bytes, g->stream);
+  } else {
+    if (b.off % es) { // a heap origin off its element alignment: the kernel loads whole elements
+      if ((rc = ensure_stage(0, bytes))) return rc;
+      b.off = g->stage_off[0];
+      if ((rc = launch_local_copy(local + b.off, origin, bytes, g->stream))) return rc;
+    }
+    rc = launch_accumulate(dtype, op, remote, local + b.off, count, g->stream);
+  }
+  return rc ? rc : finish(false);
+}
+
+// ---------------------------------------------------------------------------------------------
 // point to point
 // ---------------------------------------------------------------------------------------------
 static Ctx::P2PBounce* acquire_bounce() {
@@ -2267,6 +2393,18 @@ int b200mpi_allreduce_loc(const void* send, void* recv, size_t count, int dtype,
 }
 int b200mpi_reduce_loc(const void* send, void* recv, size_t count, int dtype, int op, int root, int memkind) {
   return do_allreduce_loc(send, recv, count, dtype, op, root, memkind, false);
+}
+int b200mpi_win_create(void* base, size_t bytes, int* win) { return do_win_create(base, bytes, win); }
+int b200mpi_win_free(int win) { return do_win_fence(win, true); }
+int b200mpi_win_fence(int win) { return do_win_fence(win, false); }
+int b200mpi_put(const void* origin, size_t count, int dtype, int target, size_t target_disp, int win, int memkind) {
+  return do_rma(kPut, origin, count, dtype, 0, target, target_disp, win, memkind);
+}
+int b200mpi_get(void* origin, size_t count, int dtype, int target, size_t target_disp, int win, int memkind) {
+  return do_rma(kGet, origin, count, dtype, 0, target, target_disp, win, memkind);
+}
+int b200mpi_accumulate(const void* origin, size_t count, int dtype, int op, int target, size_t target_disp, int win, int memkind) {
+  return do_rma(kAccumulate, origin, count, dtype, op, target, target_disp, win, memkind);
 }
 int b200mpi_gather(const void* send, void* recv, size_t count_per_rank, int dtype, int root, int memkind) { return do_gather(send, recv, count_per_rank, dtype, root, memkind, false); }
 int b200mpi_scatter(const void* send, void* recv, size_t count_per_rank, int dtype, int root, int memkind) { return do_gather(send, recv, count_per_rank, dtype, root, memkind, true); }

@@ -2037,9 +2037,107 @@ __global__ void scrub_kernel(Comm c) {
   else sync_end_failed(c);
 }
 
-// A device-wide rendezvous with nothing in between (b200mpi_barrier).
+// A device-wide rendezvous with nothing in between (b200mpi_barrier, and b200mpi_win_fence under its
+// own signature).
 __global__ void barrier_kernel(Comm c) {
   collective(c, 0, 0, [](const uint64_t*, const uint64_t*) {});
+}
+
+// ---------------------------------------------------------------------------------------------
+// One-sided Accumulate (b200mpi_accumulate): dst[e] = Op(dst[e], src[e]) for every element, each an
+// atomic read-modify-write at system scope, where dst is the target's window through its peer
+// mapping and src this rank's origin (or its staging block) in local HBM.  Concurrent Accumulates with
+// the same type and op from any ranks therefore combine in some order, none lost.
+//   sums and i64 max/min: fire-and-forget `red`.  f32 sum has a 16-byte form; sm_90a flushes f32
+//     atomic add inputs and results that are subnormal to zero of the same sign (there is no .noftz
+//     f32 red), so an f32 Accumulate SUM differs there from Allreduce, which keeps subnormals.
+//   f32 / f64 max and min: an atom.cas loop that applies OpMax / OpMin (b > a ? b : a), so a NaN
+//     already in the target stays and a NaN contribution is dropped; the result depends on the order
+//     of contributions only through NaNs and zeros of mixed sign.
+// ---------------------------------------------------------------------------------------------
+template <typename T, typename Op>
+struct Red { // f32 / f64 max and min
+  using Bits = std::conditional_t<sizeof(T) == 4, uint32_t, unsigned long long>;
+  __device__ __forceinline__ static void one(T* p, T v) {
+    Bits old;
+    if constexpr (sizeof(T) == 4) asm volatile("ld.relaxed.sys.global.b32 %0, [%1];" : "=r"(old) : "l"(p) : "memory");
+    else asm volatile("ld.relaxed.sys.global.b64 %0, [%1];" : "=l"(old) : "l"(p) : "memory");
+    for (;;) {
+      T cur, next;
+      memcpy(&cur, &old, sizeof(T));
+      next = Op::template apply<T>(cur, v);
+      Bits want, seen;
+      memcpy(&want, &next, sizeof(T));
+      // No early exit when want == old: only a successful compare-and-swap proves that `old` was the
+      // target's value, so the result never rests on the load above being current.
+      if constexpr (sizeof(T) == 4)
+        asm volatile("atom.relaxed.sys.global.cas.b32 %0, [%1], %2, %3;" : "=r"(seen) : "l"(p), "r"(old), "r"(want) : "memory");
+      else
+        asm volatile("atom.relaxed.sys.global.cas.b64 %0, [%1], %2, %3;" : "=l"(seen) : "l"(p), "l"(old), "l"(want) : "memory");
+      if (seen == old) return;
+      old = seen;
+    }
+  }
+};
+template <> struct Red<float, OpSum> {
+  __device__ __forceinline__ static void one(float* p, float v) {
+    asm volatile("red.relaxed.sys.global.add.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
+  }
+  __device__ __forceinline__ static void vec(float* p, const Pack<float>& v) {
+    asm volatile("red.relaxed.sys.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(v.v[0]), "f"(v.v[1]), "f"(v.v[2]), "f"(v.v[3]) : "memory");
+  }
+};
+template <> struct Red<double, OpSum> {
+  __device__ __forceinline__ static void one(double* p, double v) {
+    asm volatile("red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(p), "d"(v) : "memory");
+  }
+};
+template <> struct Red<long long, OpSum> { // wraps, as Go int64 does
+  __device__ __forceinline__ static void one(long long* p, long long v) {
+    asm volatile("red.relaxed.sys.global.add.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+  }
+};
+template <> struct Red<long long, OpMax> {
+  __device__ __forceinline__ static void one(long long* p, long long v) {
+    asm volatile("red.relaxed.sys.global.max.s64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+  }
+};
+template <> struct Red<long long, OpMin> {
+  __device__ __forceinline__ static void one(long long* p, long long v) {
+    asm volatile("red.relaxed.sys.global.min.s64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+  }
+};
+
+// One 16-byte vector: the 16-byte red where there is one (f32 sum), else one element at a time.
+template <typename T, typename Op>
+__device__ __forceinline__ void red_vec(T* p, const Pack<T>& v) {
+  if constexpr (std::is_same<T, float>::value && std::is_same<Op, OpSum>::value) {
+    Red<T, Op>::vec(p, v);
+  } else {
+#pragma unroll
+    for (int k = 0; k < Pack<T>::N; ++k) Red<T, Op>::one(p + k, v.v[k]);
+  }
+}
+
+// `count` elements; dst is element aligned (checked by the host), src element aligned too (a heap
+// origin that is not is staged first).  The target is split at its first 16-byte boundary (split16):
+// head and tail elements one at a time, the whole vectors between them 16 bytes at a time when src
+// has dst's residue mod 16, otherwise every element one at a time.  Grid-strided: a capped grid
+// (b200mpi_set_max_blocks) makes several passes.
+template <typename T, typename Op>
+__global__ void __launch_bounds__(256, 1)
+accumulate_kernel(T* dst, const T* __restrict__ src, size_t count) {
+  const size_t tid = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  constexpr int EPV = Pack<T>::N;
+  const bool agree = ((reinterpret_cast<uintptr_t>(dst) ^ reinterpret_cast<uintptr_t>(src)) & 15) == 0;
+  const Split16 sp = agree ? split16(reinterpret_cast<uintptr_t>(dst), count, sizeof(T)) : Split16{count, 0, 0};
+  for (size_t e = tid; e < sp.head; e += stride) Red<T, Op>::one(dst + e, src[e]);
+  T* const d = dst + sp.head;
+  const T* const s = src + sp.head;
+  unrolled<4, Pack<T>>(0, sp.nvec, [&](size_t i, Pack<T>& v) { v = ld_pack<T>(s + i * EPV); },
+                       [&](size_t i, const Pack<T>& v) { red_vec<T, Op>(d + i * EPV, v); });
+  for (size_t e = sp.head + sp.nvec * EPV + tid; e < count; e += stride) Red<T, Op>::one(dst + e, src[e]);
 }
 
 } // namespace b200

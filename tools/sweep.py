@@ -467,6 +467,64 @@ def main():
             for b in (send, recv, plain, plain_out):
                 b.free()
 
+    rma = [c for c in ("put", "get", "accumulate") if c in colls]
+    if rma:
+        # One-sided calls, blocking, heap origins, one window of max_bytes per rank; time = events around
+        # back-to-back calls, max over ranks.  Put and Get move S one way between rank and rank + 1, so
+        # every GPU sends (Put) or receives (Get) S: the bound is S over 450 GB/s per direction (H100 SXM
+        # data sheet).  Also the blocking latency of one 8-byte Put (median of 200 calls), and f32, f64 and
+        # i64 SUM Accumulate next to Put of the same size: uncontended (into rank + 1) and contended (every
+        # rank into rank 0, whose ingress then carries (n-1)*S: that is the bound there).
+        if n < 2 or L.get_param("shared_device"):
+            emit({"coll": "rma", "ok": True, "note": "fewer than two NVLink-connected GPUs (ranks %s): Put, Get and Accumulate not measured"
+                  % ("share one GPU" if n > 1 else "= 1")})
+        else:
+            per_max = min(args.max_bytes, 1 << 30)
+            wmem = mpi.Alloc(per_max, np.uint8)
+            # finite, normal origin values for every dtype read from it: f64 1.0, as f32 0.0 and 1.875
+            org = mpi.Alloc(per_max // 8, np.float64).copy_from_host(np.ones(per_max // 8))
+            w = mpi.WinCreate(wmem)
+            nxt = (rank + 1) % n
+            link = 450e9
+
+            def rma_call(fn, *a):
+                def call():
+                    if fn(*a):
+                        raise RuntimeError(L.last_error())
+                return call
+            ts = []
+            for i in range(220):
+                mpi.Barrier() if i % 50 == 0 else None
+                t0 = time.perf_counter()
+                rma_call(lib.b200mpi_put, org.ptr, 1, L.F64, nxt, 0, w.id, L.DEVICE)()
+                ts.append(time.perf_counter() - t0)
+            w.Fence()
+            emit({"coll": "put", "dtype": "f64", "bytes": 8, "t_call_us_median": maxr(sorted(ts[20:])[100]) * 1e6, "ok": True})
+            for S in [s for s in sizes if s <= per_max]:
+                it, wm = iters_for(S)
+                t_put = None
+                for coll in [c for c in ("put", "get") if c in rma]:
+                    fn = lib.b200mpi_put if coll == "put" else lib.b200mpi_get
+                    t = timed(rma_call(fn, org.ptr, S, L.U8, nxt, 0, w.id, L.DEVICE), it, wm)
+                    w.Fence()
+                    t_put = t if coll == "put" else t_put
+                    emit({"coll": coll, "dtype": "u8", "bytes": S, "t_us": t * 1e6, "algbw_gbs": S / t / 1e9,
+                          "link_roofline_share": S / link / t, "ok": True})
+                if "accumulate" in rma:
+                    for dn, code, es in (("f32", L.F32, 4), ("f64", L.F64, 8), ("i64", L.I64, 8)):
+                        for shape, target in (("uncontended", nxt), ("contended", 0)):
+                            t = timed(rma_call(lib.b200mpi_accumulate, org.ptr, S // es, code, L.SUM, target, 0, w.id, L.DEVICE), it, wm)
+                            w.Fence()
+                            bound = S / link if shape == "uncontended" else (n - 1) * S / link
+                            row = {"coll": "accumulate", "dtype": dn, "algo": shape, "bytes": S, "t_us": t * 1e6,
+                                   "algbw_gbs": S / t / 1e9, "link_roofline_share": bound / t, "ok": True}
+                            if t_put is not None:
+                                row["vs_put"] = t_put / t
+                            emit(row)
+            w.Free()
+            wmem.free()
+            org.free()
+
     if "p2p" in colls and n > 1:
         # bounce (examples/bounce/bounce.go:85-138): even sends, odd returns; device-resident float64
         maxp = min(args.max_bytes, 256 << 20)

@@ -846,6 +846,106 @@ func (w *cudaWindow) Free() error {
 	return nil
 }
 
+// cudaWindow is also a PassiveWindow.
+var _ PassiveWindow = (*cudaWindow)(nil)
+
+func (w *cudaWindow) Lock(target int, lockType LockType) error {
+	if lockType != LockExclusive && lockType != LockShared {
+		return errors.New("mpi: lock type must be LockExclusive or LockShared")
+	}
+	if rc := C.b200mpi_win_lock(C.int(lockType), C.int(target), w.id); rc != 0 {
+		return lastError(rc, 0)
+	}
+	return nil
+}
+
+func (w *cudaWindow) Unlock(target int) error {
+	if rc := C.b200mpi_win_unlock(C.int(target), w.id); rc != 0 {
+		return lastError(rc, 0)
+	}
+	return nil
+}
+
+// GetAccumulate: result must match origin's element type, length and memory kind (origin may be nil
+// for NoOp).
+func (w *cudaWindow) GetAccumulate(origin, result interface{}, target, disp int, op Op) error {
+	rp, n, dt, mk, err := lowerOrigin("GetAccumulate", result, disp)
+	if err != nil {
+		return err
+	}
+	var optr unsafe.Pointer
+	if origin != nil {
+		p, on, odt, omk, err := lowerOrigin("GetAccumulate", origin, disp)
+		if err != nil {
+			return err
+		}
+		if on != n || odt != dt || omk != mk {
+			return errors.New("mpi: GetAccumulate origin and result must have the same length, type and memory kind")
+		}
+		optr = p
+	} else if op != NoOp {
+		return errors.New("mpi: GetAccumulate needs an origin unless op is NoOp")
+	}
+	if rc := C.b200mpi_get_accumulate(optr, rp, C.size_t(n), dt, C.int(op), C.int(target), C.size_t(disp), w.id, mk); rc != 0 {
+		return lastError(rc, 0)
+	}
+	return nil
+}
+
+// FetchAndOp: value is a float32, float64 or int64 (an int is taken as int64); the previous value
+// comes back with the same type. One kernel launch, no staging.
+func (w *cudaWindow) FetchAndOp(value interface{}, target, disp int, op Op) (interface{}, error) {
+	if disp < 0 {
+		return nil, errors.New("mpi: FetchAndOp displacement must be >= 0")
+	}
+	if v, ok := value.(int); ok {
+		value = int64(v)
+	}
+	var origin unsafe.Pointer
+	var dt C.int
+	var ret interface{}
+	var result unsafe.Pointer
+	switch v := value.(type) {
+	case float32:
+		r := new(float32)
+		origin, dt, ret, result = unsafe.Pointer(&v), C.B200MPI_F32, r, unsafe.Pointer(r)
+	case float64:
+		r := new(float64)
+		origin, dt, ret, result = unsafe.Pointer(&v), C.B200MPI_F64, r, unsafe.Pointer(r)
+	case int64:
+		r := new(int64)
+		origin, dt, ret, result = unsafe.Pointer(&v), C.B200MPI_I64, r, unsafe.Pointer(r)
+	default:
+		return nil, fmt.Errorf("mpi: FetchAndOp takes a float32, float64 or int64, not %T", value)
+	}
+	if op == NoOp {
+		origin = nil
+	}
+	if rc := C.b200mpi_fetch_and_op(origin, result, dt, C.int(op), C.int(target), C.size_t(disp), w.id); rc != 0 {
+		return nil, lastError(rc, 0)
+	}
+	switch r := ret.(type) {
+	case *float32:
+		return *r, nil
+	case *float64:
+		return *r, nil
+	default:
+		return *(r.(*int64)), nil
+	}
+}
+
+func (w *cudaWindow) CompareAndSwap(value, compare int64, target, disp int) (int64, error) {
+	if disp < 0 {
+		return 0, errors.New("mpi: CompareAndSwap displacement must be >= 0")
+	}
+	var old int64
+	if rc := C.b200mpi_compare_and_swap(unsafe.Pointer(&value), unsafe.Pointer(&compare), unsafe.Pointer(&old), C.B200MPI_I64,
+		C.int(target), C.size_t(disp), w.id); rc != 0 {
+		return 0, lastError(rc, 0)
+	}
+	return old, nil
+}
+
 // Scatterv: root always sends its table with one small Bcast, so the other ranks may pass nil.
 func (c *Cuda) Scatterv(send, recv interface{}, counts []int, root int) ([]int, error) {
 	n, isRoot := c.Size(), c.Rank() == root

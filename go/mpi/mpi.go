@@ -31,6 +31,7 @@
 //	ReduceScatterv                    ReduceScatter with a different block length for every rank
 //	AllreduceLoc, ReduceLoc           MAXLOC / MINLOC: the best value across ranks and where it came from
 //	WinCreate -> Window               one-sided Put, Get and Accumulate into other ranks' heap memory, completed by Fence
+//	PassiveWindow                     Lock, Unlock, GetAccumulate, FetchAndOp, CompareAndSwap (type-assert the Window)
 //	Isend + Wait   the non-blocking Send design the reference sketches and comments out (mpi.go:132-152)
 //
 // They are served through the optional Collective interface, the upgrade the reference hints at
@@ -56,6 +57,16 @@ const (
 	Sum Op = iota
 	Max
 	Min
+	Replace // one-sided calls only: the target takes origin's value
+	NoOp    // GetAccumulate and FetchAndOp only: the target is left as it is (an atomic read)
+)
+
+// LockType selects the lock PassiveWindow.Lock takes on a target's window.
+type LockType int
+
+const (
+	LockExclusive LockType = 1 // excludes every other holder
+	LockShared    LockType = 2 // excludes exclusive holders only
 )
 
 // Collective is implemented by transports that offer collectives natively.
@@ -132,6 +143,28 @@ type Window interface {
 	Accumulate(origin interface{}, target, disp int, op Op) error
 	Fence() error
 	Free() error
+}
+
+// PassiveWindow is a Window with passive-target synchronisation and atomic fetches (MPI-3). Window
+// itself is unchanged, so other implementations of it still compile; reach these with a type
+// assertion, w.(PassiveWindow). None of them is collective.
+//
+// Lock blocks until this rank holds the lock on rank target's window (target may be this rank); it
+// fails with a timeout after the watchdog_ms knob, holding nothing. There is no fairness. Every call
+// has completed when it returns, so what this rank did under a lock is visible to the next holder.
+// A rank holding a lock on a window must not Fence or Free it: that call fails on every rank.
+// GetAccumulate sets result to the target's previous values and applies op (Sum, Max, Min, Replace or
+// NoOp, whose origin may be nil), one atomic per element; result has origin's type, length and
+// storage, and may be origin itself. FetchAndOp does the same for one float32, float64 or int64 value
+// and returns the previous value with its type. CompareAndSwap (int64) returns the previous value and
+// stores value if that equalled compare.
+type PassiveWindow interface {
+	Window
+	Lock(target int, lockType LockType) error
+	Unlock(target int) error
+	GetAccumulate(origin, result interface{}, target, disp int, op Op) error
+	FetchAndOp(value interface{}, target, disp int, op Op) (interface{}, error)
+	CompareAndSwap(value, compare int64, target, disp int) (int64, error)
 }
 
 // Float32Loc, Float64Loc and Int64Loc are the elements of AllreduceLoc and ReduceLoc: a value and

@@ -33,7 +33,8 @@ extern "C" {
 #define B200MPI_VERSION 200 /* 0.2.0: + isend/wait, reduce_scatter, reduce, alltoall, probes, get_param;
                                then gather, scatter, gatherv, scatterv, allgatherv, alltoallv, scan, exscan,
                                reduce_scatterv, allreduce_loc, reduce_loc, win_create, win_free, win_fence,
-                               put, get, accumulate (all additive) */
+                               put, get, accumulate, win_lock, win_unlock, get_accumulate, fetch_and_op,
+                               compare_and_swap (all additive) */
 #define B200MPI_MAX_RANKS 8 /* "the 8 GPUs of one box" */
 
 typedef enum {
@@ -43,7 +44,11 @@ typedef enum {
   B200MPI_F64 = 3  /* []float64 */
 } b200mpi_dtype;
 
-typedef enum { B200MPI_SUM = 0, B200MPI_MAX = 1, B200MPI_MIN = 2 } b200mpi_op;
+typedef enum { B200MPI_SUM = 0, B200MPI_MAX = 1, B200MPI_MIN = 2,
+               B200MPI_REPLACE = 3, /* one-sided only: target = origin */
+               B200MPI_NO_OP = 4    /* get_accumulate / fetch_and_op only: target unchanged (atomic read) */
+} b200mpi_op; /* every collective takes SUM, MAX and MIN only: REPLACE and NO_OP are B200MPI_ERR_ARG there */
+typedef enum { B200MPI_LOCK_EXCLUSIVE = 1, B200MPI_LOCK_SHARED = 2 } b200mpi_lock_type;
 
 typedef enum {
   B200MPI_HOST = 0,  /* pageable or pinned host memory (a Go slice) */
@@ -239,8 +244,8 @@ int b200mpi_put(const void* origin, size_t count, int dtype, int target, size_t 
 int b200mpi_get(void* origin, size_t count, int dtype, int target, size_t target_disp, int win, int memkind);
 /* target[e] = target[e] op origin[e], each element an atomic read-modify-write at system scope, so
  * concurrent Accumulates with the same dtype and op on overlapping elements, from any ranks, combine
- * in some order.  dtype f32, f64 or i64 (u8: B200MPI_ERR_UNSUPPORTED); op SUM, MAX or MIN (unknown:
- * B200MPI_ERR_ARG); the target element address must be a multiple of the element size
+ * in some order.  dtype f32, f64 or i64 (u8: B200MPI_ERR_UNSUPPORTED); op SUM, MAX, MIN or REPLACE
+ * (an element-wise atomic store of origin; NO_OP or unknown: B200MPI_ERR_ARG); the target element address must be a multiple of the element size
  * (B200MPI_ERR_ARG).  i64 SUM wraps; i64 MAX and MIN are exact; f64 SUM is one round-to-nearest add
  * per contribution, in an unspecified order.  f32 SUM flushes subnormals: on sm_90a an f32 atomic add
  * turns a subnormal input or result into zero of the same sign, unlike Allreduce, which keeps
@@ -248,6 +253,52 @@ int b200mpi_get(void* origin, size_t count, int dtype, int target, size_t target
  * does not depend on the order except for NaNs (a NaN in the target stays, a NaN contribution is
  * dropped) and zeros of mixed sign. */
 int b200mpi_accumulate(const void* origin, size_t count, int dtype, int op, int target, size_t target_disp, int win, int memkind);
+
+/* ---- one-sided communication, passive target: window locks and atomic fetches (MPI-3) ----------- */
+/* Every call below is blocking, is not collective, takes no barrier epoch, and runs on the caller's
+ * collective thread, like Put, Get and Accumulate.
+ *
+ * win_lock blocks until this rank holds the lock on rank target's window (target may be this rank).
+ * B200MPI_LOCK_EXCLUSIVE excludes every other holder; B200MPI_LOCK_SHARED excludes only exclusive
+ * holders.  There is no fairness: a steady stream of shared holders can starve an exclusive one (MPI
+ * promises none either).  Not granted within the watchdog_ms knob: B200MPI_ERR_TIMEOUT, and nothing
+ * is held.  B200MPI_ERR_ARG: an unknown or freed window, a bad lock type, a target out of range, or
+ * a second lock on the same (target, win) by this rank.  win_unlock releases it (B200MPI_ERR_ARG if
+ * this rank does not hold it).
+ * Ordering: every RMA call completes before it returns, so everything this rank did to the target's
+ * window before win_unlock is visible to the next rank that acquires that lock, of either type; there
+ * is no separate flush call.  The target's own kernels and copies that touch its window must hold the
+ * lock too, as MPI requires.  Put, Get and Accumulate work with or without locks.
+ * Locks and fences do not mix on one window: win_fence or win_free by a rank that holds a lock on
+ * that window returns B200MPI_ERR_ARG there and B200MPI_ERR_PEER on every other rank (in a world of
+ * one: B200MPI_ERR_ARG, nothing launched); the window stays live and the lock held, and after the
+ * unlock the next fence works. */
+int b200mpi_win_lock(int lock_type, int target, int win);
+int b200mpi_win_unlock(int target, int win);
+/* result[e] = the target element's previous value, then target[e] = target[e] op origin[e], each
+ * element one atomic read-modify-write at system scope: atomic with respect to Accumulate,
+ * Get_accumulate, Fetch_and_op and Compare_and_swap on the same element with the same dtype, whatever
+ * their ops, but not with respect to Put or Get (as in MPI).  dtype f32, f64 or i64 (u8:
+ * B200MPI_ERR_UNSUPPORTED); op SUM, MAX, MIN, REPLACE (target = origin) or NO_OP (target unchanged,
+ * origin may be NULL); anything else B200MPI_ERR_ARG.  The element rules are those of Accumulate (i64
+ * SUM wraps, f32 SUM flushes subnormal inputs and results to zero of the same sign, float MAX and
+ * MIN apply b > a ? b : a and b < a ? b : a); the fetched value is always the target's exact previous
+ * bits.  Target range and alignment checks are those of Accumulate.  result holds count elements in
+ * origin's memkind; result == origin is in place, any other overlap is B200MPI_ERR_ARG.  Origins and
+ * results outside the heap, or heap pointers off element alignment, are staged whole (origin through
+ * staging block 0, result through block 1; B200MPI_ERR_NOMEM if that does not fit). */
+int b200mpi_get_accumulate(const void* origin, void* result, size_t count, int dtype, int op,
+                           int target, size_t target_disp, int win, int memkind);
+/* get_accumulate of one element, with origin and result host pointers to one element each (no
+ * memkind; origin may be NULL for NO_OP).  The latency call: exactly one kernel launch and no staging
+ * copies. */
+int b200mpi_fetch_and_op(const void* origin, void* result, int dtype, int op,
+                         int target, size_t target_disp, int win);
+/* i64 only (f32, f64, u8: B200MPI_ERR_UNSUPPORTED): *result = the target element's old value, and
+ * *origin is stored there if that old value equals *compare; one atomic at system scope.  Host
+ * pointers to one element each, one kernel launch. */
+int b200mpi_compare_and_swap(const void* origin, const void* compare, void* result, int dtype,
+                             int target, size_t target_disp, int win);
 
 /* Enqueue-only forms on the library stream (DEVICE memkind only). */
 int b200mpi_bcast_async(void* buf, size_t count, int dtype, int root);

@@ -12,6 +12,8 @@ LIB_PATH = os.path.join(_HERE, "lib", "libb200mpi.so")
 # enums of include/b200mpi.h
 U8, I64, F32, F64 = 0, 1, 2, 3
 SUM, MAX, MIN = 0, 1, 2
+REPLACE, NO_OP = 3, 4                      # one-sided only
+LOCK_EXCLUSIVE, LOCK_SHARED = 1, 2
 HOST, DEVICE = 0, 1
 COLL_ALLREDUCE, COLL_BCAST, COLL_ALLGATHER, COLL_REDUCE_SCATTER = 0, 1, 2, 3
 ALGO_AUTO, ALGO_ONESHOT, ALGO_TWOSHOT, ALGO_RING, ALGO_NVLS, ALGO_TWOSHOT_SMEM, ALGO_LL, ALGO_HYBRID = 0, 1, 2, 3, 4, 5, 6, 7
@@ -64,6 +66,11 @@ SYMBOLS = {
     "b200mpi_put": (_c.c_int, [_c.c_void_p, _c.c_size_t, _c.c_int, _c.c_int, _c.c_size_t, _c.c_int, _c.c_int]),
     "b200mpi_get": (_c.c_int, [_c.c_void_p, _c.c_size_t, _c.c_int, _c.c_int, _c.c_size_t, _c.c_int, _c.c_int]),
     "b200mpi_accumulate": (_c.c_int, [_c.c_void_p, _c.c_size_t, _c.c_int, _c.c_int, _c.c_int, _c.c_size_t, _c.c_int, _c.c_int]),
+    "b200mpi_win_lock": (_c.c_int, [_c.c_int, _c.c_int, _c.c_int]),
+    "b200mpi_win_unlock": (_c.c_int, [_c.c_int, _c.c_int]),
+    "b200mpi_get_accumulate": (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_size_t, _c.c_int, _c.c_int, _c.c_int, _c.c_size_t, _c.c_int, _c.c_int]),
+    "b200mpi_fetch_and_op": (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_int, _c.c_int, _c.c_int, _c.c_size_t, _c.c_int]),
+    "b200mpi_compare_and_swap": (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_int, _c.c_int, _c.c_size_t, _c.c_int]),
     "b200mpi_reduce_scatter_async": (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_size_t, _c.c_int, _c.c_int]),
     "b200mpi_numa_node": (_c.c_int, []),
     "b200mpi_barrier": (_c.c_int, []),

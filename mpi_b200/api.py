@@ -13,6 +13,7 @@ Same names, same argument meaning, same blocking behaviour:
     ReduceScatterv(send, recv, counts, op)                                                   (new)
     AllreduceLoc(send, recv, op)  ReduceLoc(send, recv, op, root)   (MAXLOC / MINLOC, new)
     WinCreate(local) -> Win: Put, Get, Accumulate, Fence, Free      (one-sided, fence-synchronised, new)
+        + Lock, Unlock, GetAccumulate, FetchAndOp, CompareAndSwap   (passive target, new)
     Isend(data, destination, tag) + Wait(destination, tag)     (the Send/Wait design commented out
                                                                 in the reference, mpi.go:132-152)
 
@@ -32,6 +33,8 @@ from . import _lib as L
 from . import flags as _flags
 
 SUM, MAX, MIN = L.SUM, L.MAX, L.MIN
+REPLACE, NO_OP = L.REPLACE, L.NO_OP                      # one-sided only
+LOCK_EXCLUSIVE, LOCK_SHARED = L.LOCK_EXCLUSIVE, L.LOCK_SHARED
 
 
 class MpiError(Exception):
@@ -568,7 +571,13 @@ class Win:
     block until the origin may be reused (Get: until it holds the data).  What they write is visible
     to the target after its next Fence, which every rank calls; a location written by one rank and
     read or written by another between two fences is undefined, except by Accumulates with the same
-    type and op.  Free is a Fence that also drops the window."""
+    type and op.  Free is a Fence that also drops the window.
+
+    Passive target: Lock(target) / Unlock(target) give this rank mutual exclusion on one target's
+    window without the other ranks taking part; every call has completed when it returns, so what a
+    rank did under the lock is visible to the next holder.  GetAccumulate, FetchAndOp and
+    CompareAndSwap return the target's previous values, one atomic per element.  A rank holding a lock
+    on this window must not Fence or Free it (MpiError, and the other ranks' call fails too)."""
 
     def __init__(self, wid):
         self.id = wid
@@ -599,6 +608,70 @@ class Win:
         float32, float64 and int64 (an f32 SUM flushes subnormals to zero; see b200mpi.h)."""
         ptr, count, dt, kind = self._origin(origin, disp, "Accumulate")
         _check(L.load().b200mpi_accumulate(ptr, count, dt, int(op), int(target), int(disp), self.id, kind))
+
+    def Lock(self, target, lock_type=LOCK_EXCLUSIVE):
+        """Blocks until this rank holds the lock on rank `target`'s window (LOCK_EXCLUSIVE or
+        LOCK_SHARED); MpiError ERR_TIMEOUT if it is not granted within the watchdog_ms knob."""
+        if lock_type not in (LOCK_EXCLUSIVE, LOCK_SHARED):
+            raise ValueError("mpi: lock_type must be LOCK_EXCLUSIVE or LOCK_SHARED")
+        _check(L.load().b200mpi_win_lock(int(lock_type), int(target), self.id))
+
+    def Unlock(self, target):
+        _check(L.load().b200mpi_win_unlock(int(target), self.id))
+
+    def GetAccumulate(self, origin, result, target, disp=0, op=SUM):
+        """result[i] = target[disp + i] before, then target[disp + i] = target[disp + i] op origin[i],
+        element by element and atomically; op SUM, MAX, MIN, REPLACE or NO_OP (origin may be None).
+        result has origin's element type, length and storage (it may be origin itself); returns it."""
+        if (isinstance(result, (str, bytes)) or (isinstance(result, memoryview) and result.readonly)
+                or (isinstance(result, np.ndarray) and not result.flags["WRITEABLE"])):
+            raise TypeError("mpi: GetAccumulate needs a writable result (numpy array, bytearray or DeviceSlice)")
+        rptr, count, dt, kind = self._origin(result, disp, "GetAccumulate")
+        optr = None
+        if origin is not None:
+            optr, ocount, odt, okind = self._origin(origin, disp, "GetAccumulate")
+            if odt != dt or okind != kind:
+                raise TypeError("mpi: GetAccumulate's origin and result must have one element type and storage")
+            if ocount != count:
+                raise ValueError("mpi: GetAccumulate's origin and result must have the same length")
+        elif int(op) != NO_OP:
+            raise TypeError("mpi: GetAccumulate needs an origin unless op is NO_OP")
+        _check(L.load().b200mpi_get_accumulate(optr, rptr, count, dt, int(op), int(target), int(disp), self.id, kind))
+        return result
+
+    @staticmethod
+    def _scalar(value, what, allowed=(np.float32, np.float64, np.int64)):
+        """A one-element array of the value's numpy type (int: int64, float: float64)."""
+        if isinstance(value, (bool, np.bool_)):
+            raise TypeError("mpi: %s takes a number, not a bool" % what)
+        if isinstance(value, int):
+            value = np.int64(value)
+        elif isinstance(value, float):
+            value = np.float64(value)
+        if not isinstance(value, allowed):
+            raise TypeError("mpi: %s takes %s, not %s" % (what, " / ".join(t.__name__ for t in allowed), type(value).__name__))
+        return np.array([value], dtype=type(value))
+
+    def FetchAndOp(self, value, target, disp=0, op=SUM):
+        """One element: returns target[disp] before, then target[disp] = target[disp] op value, atomically.
+        value is an np.float32, np.float64 or np.int64 (int: int64, float: float64); the result has its type."""
+        v = self._scalar(value, "FetchAndOp")
+        if int(disp) < 0:
+            raise ValueError("mpi: FetchAndOp displacement must be >= 0")
+        res = np.zeros(1, dtype=v.dtype)
+        optr = None if int(op) == NO_OP else v.ctypes.data
+        _check(L.load().b200mpi_fetch_and_op(optr, res.ctypes.data, _NP2DT[v.dtype], int(op), int(target), int(disp), self.id))
+        return res[0]
+
+    def CompareAndSwap(self, value, compare, target, disp=0):
+        """int64: returns target[disp] before, and stores value there if that equals compare, atomically."""
+        v = self._scalar(value, "CompareAndSwap", (np.int64,))
+        c = self._scalar(compare, "CompareAndSwap", (np.int64,))
+        if int(disp) < 0:
+            raise ValueError("mpi: CompareAndSwap displacement must be >= 0")
+        res = np.zeros(1, dtype=np.int64)
+        _check(L.load().b200mpi_compare_and_swap(v.ctypes.data, c.ctypes.data, res.ctypes.data, L.I64, int(target), int(disp), self.id))
+        return res[0]
 
     def Fence(self):
         _check(L.load().b200mpi_win_fence(self.id))

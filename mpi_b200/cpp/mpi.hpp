@@ -16,7 +16,8 @@
 //   new: Recv, Bcast, Allreduce, Allgather, Barrier, ReduceScatter, Reduce, Alltoall, Isend/Wait,
 //        Gather, Scatter, Gatherv, Scatterv, Allgatherv, Alltoallv, Scan, Exscan, ReduceScatterv,
 //        AllreduceLoc, ReduceLoc (MAXLOC / MINLOC over mpi::ValLoc<V> pairs),
-//        WinCreate -> mpi::Window with Put, Get, Accumulate, Fence, Free (one-sided, fence-synchronised);
+//        WinCreate -> mpi::Window with Put, Get, Accumulate, Fence, Free (one-sided, fence-synchronised)
+//        and Lock, Unlock, GetAccumulate, FetchAndOp, CompareAndSwap (passive target);
 //        mpi::DeviceSlice<T> for heap-resident buffers
 // `data` may be std::vector<double|float|int64_t|uint8_t>, std::string (sent as bytes, the
 // "anything else is gob-encoded" path), or DeviceSlice<T>.
@@ -51,7 +52,9 @@ inline Error make_error(int rc) {
   return e;
 }
 
-enum Op { SUM = B200MPI_SUM, MAX = B200MPI_MAX, MIN = B200MPI_MIN };
+enum Op { SUM = B200MPI_SUM, MAX = B200MPI_MAX, MIN = B200MPI_MIN,
+          REPLACE = B200MPI_REPLACE, NO_OP = B200MPI_NO_OP }; // REPLACE and NO_OP: one-sided calls only
+enum LockType { LOCK_EXCLUSIVE = B200MPI_LOCK_EXCLUSIVE, LOCK_SHARED = B200MPI_LOCK_SHARED };
 using Raw = std::vector<uint8_t>; // mpi.go:75
 
 template <typename T> struct dtype_of;
@@ -209,6 +212,13 @@ struct Interface {
   virtual Error Put(Buffer, int, size_t, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Put"; return e; }
   virtual Error Get(Buffer, int, size_t, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Get"; return e; }
   virtual Error Accumulate(Buffer, Op, int, size_t, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Accumulate"; return e; }
+  // passive target: a lock on rank `target`'s window, and the fetching atomics (one element each for
+  // FetchAndOp and CompareAndSwap, through host pointers of the dtype)
+  virtual Error WinLock(int, int, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no WinLock"; return e; }
+  virtual Error WinUnlock(int, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no WinUnlock"; return e; }
+  virtual Error GetAccumulate(Buffer, Buffer, Op, int, size_t, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no GetAccumulate"; return e; }
+  virtual Error FetchAndOp(const void*, void*, int, Op, int, size_t, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no FetchAndOp"; return e; }
+  virtual Error CompareAndSwap(const void*, const void*, void*, int, int, size_t, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no CompareAndSwap"; return e; }
   // the Send/Wait pair the reference sketches and comments out (mpi.go:132-152)
   virtual Error Isend(Buffer, int, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Isend"; return e; }
   virtual Error Wait(int, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Wait"; return e; }
@@ -261,6 +271,17 @@ struct Cuda : Interface {
   Error Get(Buffer o, int target, size_t disp, int win) override { return make_error(b200mpi_get(o.ptr, o.count, o.dtype, target, disp, win, o.memkind)); }
   Error Accumulate(Buffer o, Op op, int target, size_t disp, int win) override {
     return make_error(b200mpi_accumulate(o.ptr, o.count, o.dtype, op, target, disp, win, o.memkind));
+  }
+  Error WinLock(int type, int target, int win) override { return make_error(b200mpi_win_lock(type, target, win)); }
+  Error WinUnlock(int target, int win) override { return make_error(b200mpi_win_unlock(target, win)); }
+  Error GetAccumulate(Buffer o, Buffer r, Op op, int target, size_t disp, int win) override {
+    return make_error(b200mpi_get_accumulate(o.ptr, r.ptr, r.count, r.dtype, op, target, disp, win, r.memkind));
+  }
+  Error FetchAndOp(const void* o, void* r, int dtype, Op op, int target, size_t disp, int win) override {
+    return make_error(b200mpi_fetch_and_op(o, r, dtype, op, target, disp, win));
+  }
+  Error CompareAndSwap(const void* o, const void* c, void* r, int dtype, int target, size_t disp, int win) override {
+    return make_error(b200mpi_compare_and_swap(o, c, r, dtype, target, disp, win));
   }
   Error Isend(Buffer d, int destination, int tag) override { return make_error(b200mpi_isend(d.ptr, d.count, d.dtype, destination, tag, d.memkind)); }
   Error Wait(int destination, int tag) override { return make_error(b200mpi_wait(destination, tag)); }
@@ -473,11 +494,38 @@ template <typename V> inline Error ReduceLoc(const DeviceSlice<ValLoc<V>>& send,
 // and Accumulate move the origin (a vector or DeviceSlice) to or from element `disp` of rank
 // `target`'s window, counted in the origin's element type, and return once the origin may be reused
 // (Get: holds the data).  Their writes are visible to the target after its next Fence, which every
-// rank calls; Free is a Fence that also drops the window.  Accumulate (SUM, MAX, MIN over float,
-// double and int64_t) is element-wise atomic; an f32 SUM flushes subnormals to zero (b200mpi.h).
+// rank calls; Free is a Fence that also drops the window.  Accumulate (SUM, MAX, MIN, REPLACE over
+// float, double and int64_t) is element-wise atomic; an f32 SUM flushes subnormals to zero (b200mpi.h).
+// Passive target: Lock / Unlock one target's window without the other ranks; GetAccumulate (the
+// result has the origin's type, length and storage, and may be the origin; NO_OP takes nullptr as
+// origin), FetchAndOp and CompareAndSwap (int64_t) return the target's previous values atomically.
+// A rank must not Fence or Free a window it holds a lock on.
 class Window {
  public:
   int id = -1;
+  Error Lock(int target, LockType type = LOCK_EXCLUSIVE) { return mpier()->WinLock(type, target, id); }
+  Error Unlock(int target) { return mpier()->WinUnlock(target, id); }
+  template <typename D, typename R> Error GetAccumulate(const D& origin, R* result, int target, size_t disp, Op op = SUM) {
+    const Buffer o = lower(origin), r = lower(*result);
+    if (o.dtype != r.dtype || o.count != r.count || o.memkind != r.memkind) {
+      Error e;
+      e.code = B200MPI_ERR_ARG;
+      e.msg = "GetAccumulate: origin and result differ in element type, length or storage";
+      return e;
+    }
+    return mpier()->GetAccumulate(o, r, op, target, disp, id);
+  }
+  template <typename R> Error GetAccumulate(std::nullptr_t, R* result, int target, size_t disp, Op op = NO_OP) {
+    Buffer none = lower(*result);
+    none.ptr = nullptr;
+    return mpier()->GetAccumulate(none, lower(*result), op, target, disp, id);
+  }
+  template <typename T> Error FetchAndOp(T value, T* result, int target, size_t disp, Op op = SUM) {
+    return mpier()->FetchAndOp(op == NO_OP ? nullptr : &value, result, dtype_of<T>::value, op, target, disp, id);
+  }
+  Error CompareAndSwap(int64_t value, int64_t compare, int64_t* result, int target, size_t disp) {
+    return mpier()->CompareAndSwap(&value, &compare, result, B200MPI_I64, target, disp, id);
+  }
   template <typename D> Error Put(const D& origin, int target, size_t disp) { return mpier()->Put(lower(origin), target, disp, id); }
   template <typename T> Error Get(std::vector<T>* origin, int target, size_t disp) { return mpier()->Get(lower(*origin), target, disp, id); }
   template <typename T> Error Get(DeviceSlice<T>* origin, int target, size_t disp) { return mpier()->Get(lower(*origin), target, disp, id); }

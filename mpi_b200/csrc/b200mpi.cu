@@ -167,8 +167,15 @@ struct Ctx {
   struct Win {
     bool live;
     uint64_t off[B200MPI_MAX_RANKS], bytes[B200MPI_MAX_RANKS];
+    uint32_t lock_cell;                    // its lock word in every rank's control region (kWinLockOff)
+    uint8_t held[B200MPI_MAX_RANKS];       // the lock this rank holds on each target's window: 0 none, or a b200mpi_lock_type
   };
   std::vector<Win> wins;
+  std::vector<bool> lock_cell_used;        // kWinLockCells entries, one per lock word; a freed window's cell is reused
+  // Host-mapped pinned words (allocated on first use): [0] the value fetch_and_op and compare_and_swap
+  // fetch, [1] win_lock_try_kernel's verdict.
+  uint64_t* rma_host = nullptr;
+  uint64_t* rma_dev = nullptr;
 };
 
 static_assert(kHeapReserved == kCtrlBytes, "heap.h and kernels.cuh disagree about the control region");
@@ -222,6 +229,7 @@ struct Spinner { // host-side wait with watchdog
   uint32_t it = 0;
   int64_t limit_ns;
   explicit Spinner(int64_t ns) : limit_ns(ns) {}
+  bool expired() const { return limit_ns > 0 && std::chrono::duration_cast<std::chrono::nanoseconds>(Clock::now() - t0).count() > limit_ns; }
   bool step() { // false => timed out
     if (++it < 4096) {
 #if defined(__x86_64__)
@@ -1568,17 +1576,29 @@ static int do_win_create(void* base, size_t bytes, int* win) {
   if (!win) bad = "NULL result pointer";
   else if ((base || bytes) && (!base || bytes > g->heap.size || !g->heap.contains(base, bytes, off)))
     bad = "window memory must lie in this rank's b200mpi_alloc heap (or be 0 bytes at NULL)";
-  struct { uint64_t id, off, bytes, bad; } mine = {g->wins.size(), off, bytes, bad ? 1u : 0u}, all[B200MPI_MAX_RANKS];
+  // The lowest free lock cell: create and free are collective and run in the same order on every rank,
+  // so every rank picks the same one.  This rank zeroes its own word before the exchange, so no peer
+  // can lock it before it is clear.
+  g->lock_cell_used.resize(kWinLockCells);
+  const uint64_t cell = std::find(g->lock_cell_used.begin(), g->lock_cell_used.end(), false) - g->lock_cell_used.begin();
+  if (!bad && cell < kWinLockCells) {
+    CUDA_OK(cudaMemsetAsync((char*)g->heap.base[g->ctrl.rank] + kWinLockOff + cell * kWinLockStride, 0, sizeof(uint64_t), g->stream));
+    CUDA_OK(cudaStreamSynchronize(g->stream));
+  }
+  struct { uint64_t id, off, bytes, bad, cell; } mine = {g->wins.size(), off, bytes, bad ? 1u : 0u, cell}, all[B200MPI_MAX_RANKS];
   std::string err;
   if ((rc = g->ctrl.allgather(&mine, sizeof mine, all, err, g->watchdog_ns > 0 ? g->watchdog_ns : -1))) return fail(rc, "win_create: " + err);
   if (bad) return fail(B200MPI_ERR_ARG, std::string("win_create: ") + bad);
-  Ctx::Win w = {true, {}, {}};
+  Ctx::Win w = {true, {}, {}, (uint32_t)cell, {}};
   for (int r = 0; r < g->ctrl.n; ++r) {
     if (all[r].bad) return fail(B200MPI_ERR_PEER, "win_create: rank " + std::to_string(r) + " refused its arguments");
     if (all[r].id != mine.id) return fail(B200MPI_ERR_PEER, "win_create: ranks disagree about the window id (" + std::to_string(all[r].id) + " on rank " + std::to_string(r) + ", " + std::to_string(mine.id) + " here)");
+    if (all[r].cell != cell) return fail(B200MPI_ERR_PEER, "win_create: ranks disagree about the lock cell (" + std::to_string(all[r].cell) + " on rank " + std::to_string(r) + ", " + std::to_string(cell) + " here)");
     w.off[r] = all[r].off;
     w.bytes[r] = all[r].bytes;
   }
+  if (cell >= kWinLockCells) return fail(B200MPI_ERR_NOMEM, "win_create: " + std::to_string(kWinLockCells) + " windows are live already");
+  g->lock_cell_used[cell] = true;
   g->wins.push_back(w);
   *win = (int)mine.id;
   return 0;
@@ -1586,27 +1606,62 @@ static int do_win_create(void* base, size_t bytes, int* win) {
 
 // Collective: the barrier kernel under signature 15 carrying the window id, so a fence on another
 // window or a Barrier ends as B200MPI_ERR_PEER on every rank.  A world of one synchronises the stream.
-// free: the window is dropped once the fence has succeeded.
+// free: the window is dropped once the fence has succeeded.  A rank that holds a lock on the window
+// enters under a signature with the "locked" mark (extra = 1): the mismatch ends the call on every
+// rank, as B200MPI_ERR_ARG here and B200MPI_ERR_PEER on the others, and the window and lock stay.
 static int do_win_fence(int win, bool free) {
   const char* what = free ? "win_free" : "win_fence";
   int rc = need_data_plane();
   if (rc) return rc;
-  if (!find_win(win)) return unknown_win(what);
-  if (g->ctrl.n > 1 && (rc = launch_coll(barrier_kernel, "barrier_kernel", make_sig(15, 0, 0, 0, (size_t)win), 1, 32, 0, g->stream))) return rc;
-  if ((rc = finish(false))) return rc;
-  if (free) g->wins[win].live = false;
+  Ctx::Win* w = find_win(win);
+  if (!w) return unknown_win(what);
+  const bool locked = std::any_of(w->held, w->held + B200MPI_MAX_RANKS, [](uint8_t h) { return h != 0; });
+  const std::string held = std::string(what) + ": this rank holds a lock on the window (unlock it first)";
+  if (locked && g->ctrl.n == 1) return fail(B200MPI_ERR_ARG, held);
+  if (g->ctrl.n > 1 && (rc = launch_coll(barrier_kernel, "barrier_kernel", make_sig(15, 0, locked ? 1 : 0, 0, (size_t)win), 1, 32, 0, g->stream))) return rc;
+  rc = finish(false);
+  if (locked) return fail(B200MPI_ERR_ARG, held); // also when every rank held one and the marks agreed
+  if (rc) return rc;
+  if (free) {
+    w->live = false;
+    g->lock_cell_used[w->lock_cell] = false;
+  }
   return 0;
 }
 
+// with_reduction's dispatch for the one-sided calls, which also take REPLACE and NO_OP.
+template <typename F, typename G>
+static auto with_rma_op(int dtype, int op, F&& f, G&& otherwise) {
+  auto more = [&] {
+    auto g = [&](auto t) {
+      if (op == B200MPI_REPLACE) return f(t, OpReplace{});
+      if (op == B200MPI_NO_OP) return f(t, OpNoOp{});
+      return otherwise();
+    };
+    switch (dtype) {
+      case B200MPI_F32: return g(float{});
+      case B200MPI_F64: return g(double{});
+      case B200MPI_I64: return g(0ll);
+    }
+    return otherwise();
+  };
+  return with_reduction(dtype, op, f, more);
+}
+
 static int launch_accumulate(int dtype, int op, void* dst, const void* src, size_t count, cudaStream_t s) {
-  return with_reduction(
+  auto unsupported = [] { return fail(B200MPI_ERR_UNSUPPORTED, "accumulate: unsupported dtype/op (need f32, f64 or i64 with sum/max/min/replace)"); };
+  return with_rma_op(
       dtype, op,
       [&](auto t, auto o) {
         using T = decltype(t);
-        accumulate_kernel<T, decltype(o)><<<copy_grid(count * sizeof(T)), 256, 0, s>>>((T*)dst, (const T*)src, count);
-        return launch_check("accumulate_kernel");
+        if constexpr (std::is_same<decltype(o), OpNoOp>::value) {
+          return unsupported();
+        } else {
+          accumulate_kernel<T, decltype(o)><<<copy_grid(count * sizeof(T)), 256, 0, s>>>((T*)dst, (const T*)src, count);
+          return launch_check("accumulate_kernel");
+        }
       },
-      [] { return fail(B200MPI_ERR_UNSUPPORTED, "accumulate: unsupported dtype/op (need f32, f64 or i64 with sum/max/min)"); });
+      unsupported);
 }
 
 enum RmaKind { kPut, kGet, kAccumulate };
@@ -1625,7 +1680,7 @@ static int do_rma(RmaKind kind, const void* origin, size_t count, int dtype, int
   const size_t es = esize(dtype);
   if (es == 0) return arg("unknown dtype");
   if (kind == kAccumulate && dtype == B200MPI_U8) return fail(B200MPI_ERR_UNSUPPORTED, "accumulate: dtype must be f32, f64 or i64");
-  if (kind == kAccumulate && (op < B200MPI_SUM || op > B200MPI_MIN)) return arg("unknown op");
+  if (kind == kAccumulate && (op < B200MPI_SUM || op > B200MPI_REPLACE)) return arg("unknown op (accumulate takes sum, max, min or replace)");
   if (target < 0 || target >= g->ctrl.n) return arg("target out of range");
   if (memkind != B200MPI_HOST && memkind != B200MPI_DEVICE) return arg("bad memkind");
   if (count == 0) return 0;
@@ -1655,6 +1710,174 @@ static int do_rma(RmaKind kind, const void* origin, size_t count, int dtype, int
     rc = launch_accumulate(dtype, op, remote, local + b.off, count, g->stream);
   }
   return rc ? rc : finish(false);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Passive target: window locks and the fetching atomics.  Not collectives, no epoch.  A lock is one
+// 64-bit word per window in every rank's control region (kWinLockOff, kernels.cuh); win_lock relaunches
+// win_lock_try_kernel, whose attempts are bounded, until it reports the lock or watchdog_ms has passed,
+// so a waiting rank neither trips the device watchdog nor takes the collectives' resync path.  Every
+// call ends in a stream synchronisation, so everything this rank did to a window before win_unlock has
+// completed when the unlock kernel's release runs (DESIGN §3).
+// ---------------------------------------------------------------------------------------------
+static int need_rma_words() {
+  if (g->rma_host) return 0;
+  void* p = nullptr;
+  if (cudaHostAlloc(&p, 64, cudaHostAllocMapped) != cudaSuccess) { (void)cudaGetLastError(); return fail(B200MPI_ERR_CUDA, "rma: mapped result words could not be allocated"); }
+  if (cudaHostGetDevicePointer((void**)&g->rma_dev, p, 0) != cudaSuccess) { (void)cudaGetLastError(); cudaFreeHost(p); return fail(B200MPI_ERR_CUDA, "rma: mapped result words have no device address"); }
+  g->rma_host = (uint64_t*)p;
+  return 0;
+}
+
+static unsigned long long* lock_word(const Ctx::Win* w, int target) {
+  return (unsigned long long*)((char*)g->heap.base[target] + kWinLockOff + (size_t)w->lock_cell * kWinLockStride);
+}
+
+static int do_win_lock(int lock_type, int target, int win) {
+  int rc = need_data_plane();
+  if (rc) return rc;
+  Ctx::Win* w = find_win(win);
+  if (!w) return unknown_win("win_lock");
+  if (lock_type != B200MPI_LOCK_EXCLUSIVE && lock_type != B200MPI_LOCK_SHARED) return fail(B200MPI_ERR_ARG, "win_lock: lock type must be exclusive or shared");
+  if (target < 0 || target >= g->ctrl.n) return fail(B200MPI_ERR_ARG, "win_lock: target out of range");
+  if (w->held[target]) return fail(B200MPI_ERR_ARG, "win_lock: this rank already holds a lock on the target's window");
+  if ((rc = need_rma_words())) return rc;
+  volatile uint32_t* verdict = (volatile uint32_t*)(g->rma_host + 1);
+  Spinner sp(g->watchdog_ns);
+  for (;;) {
+    *verdict = 2;
+    win_lock_try_kernel<<<1, 1, 0, g->stream>>>(lock_word(w, target), lock_type == B200MPI_LOCK_EXCLUSIVE, (uint32_t*)(g->rma_dev + 1));
+    if ((rc = launch_check("win_lock_try_kernel")) || (rc = finish(false))) return rc;
+    if (*verdict == 1) break;
+    if (sp.expired()) return fail(B200MPI_ERR_TIMEOUT, "win_lock: the lock was not granted within watchdog_ms");
+  }
+  w->held[target] = (uint8_t)lock_type;
+  return 0;
+}
+
+static int do_win_unlock(int target, int win) {
+  int rc = need_data_plane();
+  if (rc) return rc;
+  Ctx::Win* w = find_win(win);
+  if (!w) return unknown_win("win_unlock");
+  if (target < 0 || target >= g->ctrl.n) return fail(B200MPI_ERR_ARG, "win_unlock: target out of range");
+  if (!w->held[target]) return fail(B200MPI_ERR_ARG, "win_unlock: this rank holds no lock on the target's window");
+  win_unlock_kernel<<<1, 1, 0, g->stream>>>(lock_word(w, target), w->held[target] == B200MPI_LOCK_EXCLUSIVE);
+  if ((rc = launch_check("win_unlock_kernel")) || (rc = finish(false))) return rc;
+  w->held[target] = 0;
+  return 0;
+}
+
+// The checks every fetching call makes first, in do_rma's order: the data plane, the window, the
+// dtype, the op, the target; then (count > 0) the range and the element alignment of the target.
+// `remote` is the target element through its peer mapping.  i64_only: compare_and_swap.
+static int rma_atomic_target(const char* what, int dtype, int op, int target, size_t target_disp, size_t count, int win, char*& remote, bool i64_only = false) {
+  int rc = need_data_plane();
+  if (rc) return rc;
+  auto arg = [&](const char* msg) { return fail(B200MPI_ERR_ARG, std::string(what) + ": " + msg); };
+  const Ctx::Win* w = find_win(win);
+  if (!w) return unknown_win(what);
+  const size_t es = esize(dtype);
+  if (es == 0) return arg("unknown dtype");
+  if (dtype == B200MPI_U8 || (i64_only && dtype != B200MPI_I64)) return fail(B200MPI_ERR_UNSUPPORTED, std::string(what) + (i64_only ? ": dtype must be i64" : ": dtype must be f32, f64 or i64"));
+  if (op < B200MPI_SUM || op > B200MPI_NO_OP) return arg("unknown op");
+  if (target < 0 || target >= g->ctrl.n) return arg("target out of range");
+  if (count == 0) return 0;
+  if (target_disp > SIZE_MAX - count || target_disp + count > w->bytes[target] / es) return arg("target_disp + count elements exceed the target's window");
+  const uint64_t at = w->off[target] + target_disp * es;
+  if (at % es) return arg("target element address is not a multiple of the element size");
+  remote = (char*)g->heap.base[target] + at;
+  return 0;
+}
+
+// result[e] = target[e] before, target[e] = target[e] op origin[e].  Origin through staging block 0 and
+// result through block 1 when they lie outside the heap or off their element alignment; result ==
+// origin shares the origin's place.
+static int do_get_accumulate(const void* origin, void* result, size_t count, int dtype, int op, int target, size_t target_disp, int win, int memkind) {
+  const char* what = "get_accumulate";
+  char* remote = nullptr;
+  int rc = rma_atomic_target(what, dtype, op, target, target_disp, count, win, remote);
+  if (rc) return rc;
+  auto arg = [&](const char* msg) { return fail(B200MPI_ERR_ARG, std::string(what) + ": " + msg); };
+  if (memkind != B200MPI_HOST && memkind != B200MPI_DEVICE) return arg("bad memkind");
+  if (count == 0) return 0;
+  const bool reads = op != B200MPI_NO_OP;
+  if (reads && !origin) return arg("NULL origin with count > 0");
+  if (!result) return arg("NULL result with count > 0");
+  const size_t es = esize(dtype), bytes = count * es;
+  const bool in_place = reads && result == origin;
+  if (reads && !in_place && (uintptr_t)result < (uintptr_t)origin + bytes && (uintptr_t)origin < (uintptr_t)result + bytes)
+    return arg("result overlaps origin without being it");
+  char* const local = (char*)g->heap.base[g->ctrl.rank];
+  Buf src, res;
+  if (reads) {
+    if ((rc = resolve(origin, bytes, memkind, 0, true, src))) return rc;
+    if (src.off % es) { // a heap origin off its element alignment: the kernel loads whole elements
+      if ((rc = ensure_stage(0, bytes))) return rc;
+      src = {g->stage_off[0], true};
+      if ((rc = launch_local_copy(local + src.off, origin, bytes, g->stream))) return rc;
+    }
+  }
+  if (in_place) {
+    res = src;
+  } else {
+    if ((rc = resolve(result, bytes, memkind, 1, false, res))) return rc;
+    if (res.off % es) {
+      if ((rc = ensure_stage(1, bytes))) return rc;
+      res = {g->stage_off[1], true};
+    }
+  }
+  rc = with_rma_op(
+      dtype, op,
+      [&](auto t, auto o) {
+        using T = decltype(t);
+        get_accumulate_kernel<T, decltype(o)><<<copy_grid(bytes), 256, 0, g->stream>>>((T*)remote, reads ? (const T*)(local + src.off) : nullptr, (T*)(local + res.off), count);
+        return launch_check("get_accumulate_kernel");
+      },
+      [&] { return arg("unknown op"); });
+  if (rc) return rc;
+  return finish(false, Staging{0, res.off, res.staged ? result : nullptr, bytes, memkind});
+}
+
+// One element between host values: the operand as a kernel parameter, the old value through the
+// mapped word.  One launch, no staging.
+static int do_fetch_and_op(const void* origin, void* result, int dtype, int op, int target, size_t target_disp, int win) {
+  const char* what = "fetch_and_op";
+  char* remote = nullptr;
+  int rc = rma_atomic_target(what, dtype, op, target, target_disp, 1, win, remote);
+  if (rc) return rc;
+  if (!origin && op != B200MPI_NO_OP) return fail(B200MPI_ERR_ARG, "fetch_and_op: NULL origin");
+  if (!result) return fail(B200MPI_ERR_ARG, "fetch_and_op: NULL result");
+  if ((rc = need_rma_words())) return rc;
+  const size_t es = esize(dtype);
+  rc = with_rma_op(
+      dtype, op,
+      [&](auto t, auto o) {
+        using T = decltype(t);
+        T v{};
+        if (op != B200MPI_NO_OP) memcpy(&v, origin, sizeof(T));
+        fetch_op_kernel<T, decltype(o)><<<1, 1, 0, g->stream>>>((T*)remote, v, (T*)g->rma_dev);
+        return launch_check("fetch_op_kernel");
+      },
+      [] { return fail(B200MPI_ERR_ARG, "fetch_and_op: unknown op"); });
+  if (rc || (rc = finish(false))) return rc;
+  memcpy(result, (const void*)g->rma_host, es);
+  return 0;
+}
+
+static int do_compare_and_swap(const void* origin, const void* compare, void* result, int dtype, int target, size_t target_disp, int win) {
+  char* remote = nullptr;
+  int rc = rma_atomic_target("compare_and_swap", dtype, B200MPI_REPLACE, target, target_disp, 1, win, remote, true);
+  if (rc) return rc;
+  if (!origin || !compare || !result) return fail(B200MPI_ERR_ARG, "compare_and_swap: NULL origin, compare or result");
+  if ((rc = need_rma_words())) return rc;
+  unsigned long long v, c;
+  memcpy(&v, origin, 8);
+  memcpy(&c, compare, 8);
+  cas_kernel<<<1, 1, 0, g->stream>>>((unsigned long long*)remote, c, v, (unsigned long long*)g->rma_dev);
+  if ((rc = launch_check("cas_kernel")) || (rc = finish(false))) return rc;
+  memcpy(result, (const void*)g->rma_host, 8);
+  return 0;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -2062,7 +2285,7 @@ static void teardown() {
   for (cudaEvent_t e : g->pipe_events) cudaEventDestroy(e);
   for (cudaEvent_t e : {g->ev0, g->ev1}) if (e) cudaEventDestroy(e);
   if (g->pool.running()) g->pool.shutdown(); // its threads fill the bounce ring
-  for (void* p : {(void*)g->bounce, (void*)g->status_host, (void*)g->ll_host}) if (p) cudaFreeHost(p);
+  for (void* p : {(void*)g->bounce, (void*)g->status_host, (void*)g->ll_host, (void*)g->rma_host}) if (p) cudaFreeHost(p);
   for (auto& b : g->p2p_bounce) if (b.host) cudaFreeHost(b.host);
   if (g->box) munmap(g->box, sizeof(Mailbox));
   {
@@ -2405,6 +2628,17 @@ int b200mpi_get(void* origin, size_t count, int dtype, int target, size_t target
 }
 int b200mpi_accumulate(const void* origin, size_t count, int dtype, int op, int target, size_t target_disp, int win, int memkind) {
   return do_rma(kAccumulate, origin, count, dtype, op, target, target_disp, win, memkind);
+}
+int b200mpi_win_lock(int lock_type, int target, int win) { return do_win_lock(lock_type, target, win); }
+int b200mpi_win_unlock(int target, int win) { return do_win_unlock(target, win); }
+int b200mpi_get_accumulate(const void* origin, void* result, size_t count, int dtype, int op, int target, size_t target_disp, int win, int memkind) {
+  return do_get_accumulate(origin, result, count, dtype, op, target, target_disp, win, memkind);
+}
+int b200mpi_fetch_and_op(const void* origin, void* result, int dtype, int op, int target, size_t target_disp, int win) {
+  return do_fetch_and_op(origin, result, dtype, op, target, target_disp, win);
+}
+int b200mpi_compare_and_swap(const void* origin, const void* compare, void* result, int dtype, int target, size_t target_disp, int win) {
+  return do_compare_and_swap(origin, compare, result, dtype, target, target_disp, win);
 }
 int b200mpi_gather(const void* send, void* recv, size_t count_per_rank, int dtype, int root, int memkind) { return do_gather(send, recv, count_per_rank, dtype, root, memkind, false); }
 int b200mpi_scatter(const void* send, void* recv, size_t count_per_rank, int dtype, int root, int memkind) { return do_gather(send, recv, count_per_rank, dtype, root, memkind, true); }

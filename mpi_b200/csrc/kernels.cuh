@@ -8,6 +8,7 @@
 // The first kCtrlBytes of each heap are control words:
 //     Slot slots[kMaxBlocks][kMaxRanks]   cross-rank flag + per-call buffer descriptor
 //     u32  ring[kMaxBlocks]               ring step counters
+//     LL cells (kLLOff), window lock words (kWinLockOff)
 // A collective kernel is   sync_start -> body -> sync_end   where both syncs are per-CTA
 // barriers between the CTAs with the same blockIdx on every rank (flag writes with
 // st.release.sys into the peer's slot, ld.acquire.sys spins on the own slot).  sync_start also
@@ -415,6 +416,9 @@ struct OpMax {
 struct OpMin {
   template <typename T> __device__ __forceinline__ static T apply(T a, T b) { return b < a ? b : a; }
 };
+// One-sided only (B200MPI_REPLACE, B200MPI_NO_OP): tags for Red and Fetch, never reduced with apply.
+struct OpReplace {};
+struct OpNoOp {};
 
 // A value-location pair of MAXLOC / MINLOC: the C struct { V val; int64_t loc; }, 16 bytes for f32,
 // f64 and i64 alike (4 padding bytes follow an f32 value).  `w` holds the value's bytes and the
@@ -2051,6 +2055,7 @@ __global__ void barrier_kernel(Comm c) {
 //   sums and i64 max/min: fire-and-forget `red`.  f32 sum has a 16-byte form; sm_90a flushes f32
 //     atomic add inputs and results that are subnormal to zero of the same sign (there is no .noftz
 //     f32 red), so an f32 Accumulate SUM differs there from Allreduce, which keeps subnormals.
+//   replace (B200MPI_REPLACE): an element-wise st.relaxed.sys.
 //   f32 / f64 max and min: an atom.cas loop that applies OpMax / OpMin (b > a ? b : a), so a NaN
 //     already in the target stays and a NaN contribution is dropped; the result depends on the order
 //     of contributions only through NaNs and zeros of mixed sign.
@@ -2058,7 +2063,9 @@ __global__ void barrier_kernel(Comm c) {
 template <typename T, typename Op>
 struct Red { // f32 / f64 max and min
   using Bits = std::conditional_t<sizeof(T) == 4, uint32_t, unsigned long long>;
-  __device__ __forceinline__ static void one(T* p, T v) {
+  __device__ __forceinline__ static void one(T* p, T v) { (void)fetch(p, v); }
+  // The CAS loop; returns the value its successful compare-and-swap saw (Get_accumulate's result).
+  __device__ __forceinline__ static T fetch(T* p, T v) {
     Bits old;
     if constexpr (sizeof(T) == 4) asm volatile("ld.relaxed.sys.global.b32 %0, [%1];" : "=r"(old) : "l"(p) : "memory");
     else asm volatile("ld.relaxed.sys.global.b64 %0, [%1];" : "=l"(old) : "l"(p) : "memory");
@@ -2074,7 +2081,7 @@ struct Red { // f32 / f64 max and min
         asm volatile("atom.relaxed.sys.global.cas.b32 %0, [%1], %2, %3;" : "=r"(seen) : "l"(p), "r"(old), "r"(want) : "memory");
       else
         asm volatile("atom.relaxed.sys.global.cas.b64 %0, [%1], %2, %3;" : "=l"(seen) : "l"(p), "l"(old), "l"(want) : "memory");
-      if (seen == old) return;
+      if (seen == old) return cur;
       old = seen;
     }
   }
@@ -2108,6 +2115,20 @@ template <> struct Red<long long, OpMin> {
   }
 };
 
+template <typename T> struct Red<T, OpReplace> { // MPI_REPLACE: an element-wise atomic store
+  __device__ __forceinline__ static void one(T* p, T v) {
+    if constexpr (sizeof(T) == 4) {
+      uint32_t b;
+      memcpy(&b, &v, 4);
+      asm volatile("st.relaxed.sys.global.b32 [%0], %1;" ::"l"(p), "r"(b) : "memory");
+    } else {
+      unsigned long long b;
+      memcpy(&b, &v, 8);
+      asm volatile("st.relaxed.sys.global.b64 [%0], %1;" ::"l"(p), "l"(b) : "memory");
+    }
+  }
+};
+
 // One 16-byte vector: the 16-byte red where there is one (f32 sum), else one element at a time.
 template <typename T, typename Op>
 __device__ __forceinline__ void red_vec(T* p, const Pack<T>& v) {
@@ -2138,6 +2159,163 @@ accumulate_kernel(T* dst, const T* __restrict__ src, size_t count) {
   unrolled<4, Pack<T>>(0, sp.nvec, [&](size_t i, Pack<T>& v) { v = ld_pack<T>(s + i * EPV); },
                        [&](size_t i, const Pack<T>& v) { red_vec<T, Op>(d + i * EPV, v); });
   for (size_t e = sp.head + sp.nvec * EPV + tid; e < count; e += stride) Red<T, Op>::one(dst + e, src[e]);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Passive target (b200mpi_get_accumulate, _fetch_and_op, _compare_and_swap, _win_lock / _unlock).
+// Fetch<T, Op>::one(p, v) is one fetching atomic at system scope that applies Op and returns the
+// element's previous bits: atom.add (f32, f64, u64), atom.max / min.s64, Red's CAS loop for float max
+// and min, atom.exch for REPLACE, an ld.relaxed.sys for NO_OP.  The same instruction at the same
+// address and width as Accumulate's red, so the two are atomic with respect to each other.  atom.add.f32
+// flushes subnormal inputs and results, as red does; the value it returns is the old bits as stored.
+// ---------------------------------------------------------------------------------------------
+template <typename T, typename Op>
+struct Fetch { // f32 / f64 max and min
+  __device__ __forceinline__ static T one(T* p, T v) { return Red<T, Op>::fetch(p, v); }
+};
+template <> struct Fetch<float, OpSum> {
+  __device__ __forceinline__ static float one(float* p, float v) {
+    float old;
+    asm volatile("atom.relaxed.sys.global.add.f32 %0, [%1], %2;" : "=f"(old) : "l"(p), "f"(v) : "memory");
+    return old;
+  }
+};
+template <> struct Fetch<double, OpSum> {
+  __device__ __forceinline__ static double one(double* p, double v) {
+    double old;
+    asm volatile("atom.relaxed.sys.global.add.f64 %0, [%1], %2;" : "=d"(old) : "l"(p), "d"(v) : "memory");
+    return old;
+  }
+};
+template <> struct Fetch<long long, OpSum> { // wraps
+  __device__ __forceinline__ static long long one(long long* p, long long v) {
+    long long old;
+    asm volatile("atom.relaxed.sys.global.add.u64 %0, [%1], %2;" : "=l"(old) : "l"(p), "l"(v) : "memory");
+    return old;
+  }
+};
+template <> struct Fetch<long long, OpMax> {
+  __device__ __forceinline__ static long long one(long long* p, long long v) {
+    long long old;
+    asm volatile("atom.relaxed.sys.global.max.s64 %0, [%1], %2;" : "=l"(old) : "l"(p), "l"(v) : "memory");
+    return old;
+  }
+};
+template <> struct Fetch<long long, OpMin> {
+  __device__ __forceinline__ static long long one(long long* p, long long v) {
+    long long old;
+    asm volatile("atom.relaxed.sys.global.min.s64 %0, [%1], %2;" : "=l"(old) : "l"(p), "l"(v) : "memory");
+    return old;
+  }
+};
+template <typename T> struct Fetch<T, OpReplace> {
+  __device__ __forceinline__ static T one(T* p, T v) {
+    T r;
+    if constexpr (sizeof(T) == 4) {
+      uint32_t b, old;
+      memcpy(&b, &v, 4);
+      asm volatile("atom.relaxed.sys.global.exch.b32 %0, [%1], %2;" : "=r"(old) : "l"(p), "r"(b) : "memory");
+      memcpy(&r, &old, 4);
+    } else {
+      unsigned long long b, old;
+      memcpy(&b, &v, 8);
+      asm volatile("atom.relaxed.sys.global.exch.b64 %0, [%1], %2;" : "=l"(old) : "l"(p), "l"(b) : "memory");
+      memcpy(&r, &old, 8);
+    }
+    return r;
+  }
+};
+template <typename T> struct Fetch<T, OpNoOp> { // an atomic read
+  __device__ __forceinline__ static T one(T* p, T) {
+    T r;
+    if constexpr (sizeof(T) == 4) {
+      uint32_t old;
+      asm volatile("ld.relaxed.sys.global.b32 %0, [%1];" : "=r"(old) : "l"(p) : "memory");
+      memcpy(&r, &old, 4);
+    } else {
+      unsigned long long old;
+      asm volatile("ld.relaxed.sys.global.b64 %0, [%1];" : "=l"(old) : "l"(p) : "memory");
+      memcpy(&r, &old, 8);
+    }
+    return r;
+  }
+};
+
+// res[e] = dst[e] before, dst[e] = Op(dst[e], src[e]), one element per thread, grid-strided over
+// copy_grid.  dst (the target through its peer mapping), src and res are element aligned (the host
+// stages misaligned heap buffers); res == src is in place (each thread reads its src element before
+// it writes that res element); src is not read for NO_OP and may be null then.  No vector form:
+// these calls are latency-bound.
+template <typename T, typename Op>
+__global__ void __launch_bounds__(256, 1)
+get_accumulate_kernel(T* dst, const T* src, T* res, size_t count) {
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < count; e += stride) {
+    T v{};
+    if constexpr (!std::is_same<Op, OpNoOp>::value) v = src[e];
+    res[e] = Fetch<T, Op>::one(dst + e, v);
+  }
+}
+
+// One element, the operand as a parameter and the old value to *out, a host-mapped word
+// (b200mpi_fetch_and_op: one launch, no staging).  One thread.
+template <typename T, typename Op>
+__global__ void fetch_op_kernel(T* dst, T v, T* out) {
+  *(volatile T*)out = Fetch<T, Op>::one(dst, v);
+}
+
+// b200mpi_compare_and_swap: *out = old; dst = v if old == cmp.  One thread, i64 only.
+__global__ void cas_kernel(unsigned long long* dst, unsigned long long cmp, unsigned long long v, unsigned long long* out) {
+  unsigned long long old;
+  asm volatile("atom.relaxed.sys.global.cas.b64 %0, [%1], %2, %3;" : "=l"(old) : "l"(dst), "l"(cmp), "l"(v) : "memory");
+  *(volatile unsigned long long*)out = old;
+}
+
+// Window locks: one 64-bit word per live window in every rank's control region, past the LL cells.
+// Bit 32 is the exclusive holder, the low 32 bits count shared holders (and shared attempts in
+// passing, which back out when they find the exclusive bit).
+//   exclusive acquire: atom.cas.acquire.sys from 0;      release: atom.and.release.sys of ~bit 32
+//     (only its own bit: a shared attempt may have incremented the count in passing)
+//   shared acquire: atom.add.acquire.sys of +1, backed out and retried if the exclusive bit was set;
+//     release: atom.add.release.sys of -1
+constexpr size_t kWinLockOff = 9u << 20;
+constexpr size_t kWinLockStride = 64;
+constexpr uint32_t kWinLockCells = 65536; // windows live at once; the table ends at 13 MiB
+constexpr unsigned long long kLockExclusive = 1ull << 32;
+static_assert(kWinLockOff >= kLLOff + kLLRegionCells * 16, "lock words overlap the LL cells");
+static_assert(kWinLockOff + (size_t)kWinLockCells * kWinLockStride <= kCtrlBytes, "lock words end past the control region");
+// Attempts one win_lock_try_kernel makes, with __nanosleep backoff from 32 ns doubling to 1 us (about
+// 0.25 ms in all), before it reports "not acquired" and the host relaunches it.  A guess, not a
+// measurement: it bounds the kernel, and the host's deadline (watchdog_ms) bounds the wait.
+constexpr int kLockAttempts = 256;
+
+// One thread: up to kLockAttempts tries at the lock word, then *acquired (host-mapped) = 1 or 0.  It
+// never spins without bound, and neither touches the device watchdog nor its status word: a rank
+// waiting on a lock is not a collective that failed.
+__global__ void win_lock_try_kernel(unsigned long long* word, int exclusive, uint32_t* acquired) {
+  unsigned ns = 32;
+  for (int i = 0; i < kLockAttempts; ++i) {
+    unsigned long long old;
+    if (exclusive) {
+      asm volatile("atom.acquire.sys.global.cas.b64 %0, [%1], %2, %3;" : "=l"(old) : "l"(word), "l"(0ull), "l"(kLockExclusive) : "memory");
+      if (old == 0) { *(volatile uint32_t*)acquired = 1; return; }
+    } else {
+      asm volatile("atom.acquire.sys.global.add.u64 %0, [%1], %2;" : "=l"(old) : "l"(word), "l"(1ull) : "memory");
+      if (!(old & kLockExclusive)) { *(volatile uint32_t*)acquired = 1; return; }
+      asm volatile("red.relaxed.sys.global.add.u64 [%0], %1;" ::"l"(word), "l"(~0ull) : "memory");
+    }
+    __nanosleep(ns);
+    if (ns < 1024) ns *= 2;
+  }
+  *(volatile uint32_t*)acquired = 0;
+}
+
+// One thread: releases what win_lock_try_kernel acquired.  The release orders this rank's earlier RMA
+// kernels before the next holder's acquire: they completed before this kernel started (DESIGN §3).
+__global__ void win_unlock_kernel(unsigned long long* word, int exclusive) {
+  unsigned long long old;
+  if (exclusive) asm volatile("atom.release.sys.global.and.b64 %0, [%1], %2;" : "=l"(old) : "l"(word), "l"(~kLockExclusive) : "memory");
+  else asm volatile("atom.release.sys.global.add.u64 %0, [%1], %2;" : "=l"(old) : "l"(word), "l"(~0ull) : "memory");
 }
 
 } // namespace b200

@@ -14,6 +14,7 @@ import argparse
 import ctypes
 import json
 import os
+import subprocess
 import sys
 import time
 
@@ -524,6 +525,83 @@ def main():
             w.Free()
             wmem.free()
             org.free()
+
+    passive = [c for c in ("lock", "fetch_and_op", "get_accumulate") if c in colls]
+    if passive:
+        # Passive target, blocking calls on a window of rank + 1 (medians of 200 calls after 20, max over
+        # ranks): an uncontended Lock + Unlock pair; one i64 Fetch_and_op SUM next to the 8-byte Put of the
+        # same window; every rank's Fetch_and_op on rank 0's counter at once, as operations per second
+        # over the world; and f64 Get_accumulate SUM of 64 MiB (heap origin and result) next to Accumulate.
+        card = {}
+        try:  # a read-only query: the numbers belong next to the card and its power limit
+            q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", str(lib.b200mpi_device())],
+                               capture_output=True, text=True, timeout=30).stdout.strip().split(", ")
+            card = {"gpu": q[0], "power_limit": q[1]} if len(q) == 2 else {}
+        except (OSError, subprocess.SubprocessError):
+            pass
+
+        def pemit(d):
+            emit(dict(d, **card))
+        if n < 2 or L.get_param("shared_device"):
+            pemit({"coll": "passive", "ok": True, "note": "fewer than two NVLink-connected GPUs (ranks %s): Lock, Fetch_and_op and "
+                  "Get_accumulate not measured" % ("share one GPU" if n > 1 else "= 1")})
+        else:
+            S = 64 << 20
+            wmem = mpi.Alloc(S // 8, np.float64).copy_from_host(np.zeros(S // 8))
+            org = mpi.Alloc(S // 8, np.float64).copy_from_host(np.ones(S // 8))
+            res = mpi.Alloc(S // 8, np.float64)
+            w = mpi.WinCreate(wmem)
+            nxt = (rank + 1) % n
+            one = np.ones(1, dtype=np.int64)
+            old = np.zeros(1, dtype=np.int64)
+
+            def median_of(call):
+                ts = []
+                for i in range(220):
+                    mpi.Barrier() if i % 50 == 0 else None
+                    t0 = time.perf_counter()
+                    if call():
+                        raise RuntimeError(L.last_error())
+                    ts.append(time.perf_counter() - t0)
+                return maxr(sorted(ts[20:])[100])
+            if "lock" in passive:
+                t = median_of(lambda: lib.b200mpi_win_lock(L.LOCK_EXCLUSIVE, nxt, w.id) or lib.b200mpi_win_unlock(nxt, w.id))
+                pemit({"coll": "lock", "algo": "exclusive_uncontended", "t_pair_us_median": t * 1e6, "ok": True})
+            if "fetch_and_op" in passive:
+                t = median_of(lambda: lib.b200mpi_fetch_and_op(one.ctypes.data, old.ctypes.data, L.I64, L.SUM, nxt, 0, w.id))
+                t_put = median_of(lambda: lib.b200mpi_put(org.ptr, 1, L.F64, nxt, 1, w.id, L.DEVICE))
+                pemit({"coll": "fetch_and_op", "dtype": "i64", "algo": "uncontended", "t_call_us_median": t * 1e6,
+                      "put_8B_t_call_us_median": t_put * 1e6, "ok": True})
+                mpi.Barrier()
+                calls = 2000
+                t0 = time.perf_counter()
+                for _ in range(calls):
+                    if lib.b200mpi_fetch_and_op(one.ctypes.data, old.ctypes.data, L.I64, L.SUM, 0, 2, w.id):
+                        raise RuntimeError(L.last_error())
+                dt = maxr(time.perf_counter() - t0)
+                mpi.Barrier()
+                final = np.zeros(1, dtype=np.int64)
+                lib.b200mpi_fetch_and_op(None, final.ctypes.data, L.I64, L.NO_OP, 0, 2, w.id)
+                pemit({"coll": "fetch_and_op", "dtype": "i64", "algo": "contended", "ops_per_s": n * calls / dt,
+                      "ok": bool(final[0] == n * calls)})
+            if "get_accumulate" in passive:
+                it, wm = iters_for(S)
+
+                def ga():
+                    if lib.b200mpi_get_accumulate(org.ptr, res.ptr, S // 8, L.F64, L.SUM, nxt, 0, w.id, L.DEVICE):
+                        raise RuntimeError(L.last_error())
+
+                def acc():
+                    if lib.b200mpi_accumulate(org.ptr, S // 8, L.F64, L.SUM, nxt, 0, w.id, L.DEVICE):
+                        raise RuntimeError(L.last_error())
+                t_ga = timed(ga, it, wm)
+                t_acc = timed(acc, it, wm)
+                pemit({"coll": "get_accumulate", "dtype": "f64", "bytes": S, "t_us": t_ga * 1e6, "algbw_gbs": S / t_ga / 1e9,
+                      "accumulate_t_us": t_acc * 1e6, "vs_accumulate": t_acc / t_ga, "ok": True})
+            w.Fence()
+            w.Free()
+            for b in (wmem, org, res):
+                b.free()
 
     if "p2p" in colls and n > 1:
         # bounce (examples/bounce/bounce.go:85-138): even sends, odd returns; device-resident float64

@@ -946,6 +946,63 @@ func (w *cudaWindow) CompareAndSwap(value, compare int64, target, disp int) (int
 	return old, nil
 }
 
+// cudaWindow is also a GroupWindow.
+var _ GroupWindow = (*cudaWindow)(nil)
+
+// cGroup: the ranks as a C int array (nil for an empty group); range and duplicates are the
+// library's to check.
+func cGroup(ranks []int) (*C.int, C.int) {
+	if len(ranks) == 0 {
+		return nil, 0
+	}
+	g := make([]C.int, len(ranks))
+	for i, r := range ranks {
+		g[i] = C.int(r)
+		if int(g[i]) != r {
+			g[i] = -1 // out of range either way
+		}
+	}
+	return &g[0], C.int(len(g))
+}
+
+func (w *cudaWindow) Post(origins []int) error {
+	p, n := cGroup(origins)
+	if rc := C.b200mpi_win_post(p, n, w.id); rc != 0 {
+		return lastError(rc, 0)
+	}
+	return nil
+}
+
+func (w *cudaWindow) Start(targets []int) error {
+	p, n := cGroup(targets)
+	if rc := C.b200mpi_win_start(p, n, w.id); rc != 0 {
+		return lastError(rc, 0)
+	}
+	return nil
+}
+
+func (w *cudaWindow) Complete() error {
+	if rc := C.b200mpi_win_complete(w.id); rc != 0 {
+		return lastError(rc, 0)
+	}
+	return nil
+}
+
+func (w *cudaWindow) Wait() error {
+	if rc := C.b200mpi_win_wait(w.id); rc != 0 {
+		return lastError(rc, 0)
+	}
+	return nil
+}
+
+func (w *cudaWindow) Test() (bool, error) {
+	var flag C.int
+	if rc := C.b200mpi_win_test(w.id, &flag); rc != 0 {
+		return false, lastError(rc, 0)
+	}
+	return flag != 0, nil
+}
+
 // Scatterv: root always sends its table with one small Bcast, so the other ranks may pass nil.
 func (c *Cuda) Scatterv(send, recv interface{}, counts []int, root int) ([]int, error) {
 	n, isRoot := c.Size(), c.Rank() == root

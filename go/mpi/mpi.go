@@ -32,6 +32,7 @@
 //	AllreduceLoc, ReduceLoc           MAXLOC / MINLOC: the best value across ranks and where it came from
 //	WinCreate -> Window               one-sided Put, Get and Accumulate into other ranks' heap memory, completed by Fence
 //	PassiveWindow                     Lock, Unlock, GetAccumulate, FetchAndOp, CompareAndSwap (type-assert the Window)
+//	GroupWindow                       Post, Start, Complete, Wait, Test: epochs between named ranks only (type-assert the Window)
 //	Isend + Wait   the non-blocking Send design the reference sketches and comments out (mpi.go:132-152)
 //
 // They are served through the optional Collective interface, the upgrade the reference hints at
@@ -165,6 +166,27 @@ type PassiveWindow interface {
 	GetAccumulate(origin, result interface{}, target, disp int, op Op) error
 	FetchAndOp(value interface{}, target, disp int, op Op) (interface{}, error)
 	CompareAndSwap(value, compare int64, target, disp int) (int64, error)
+}
+
+// GroupWindow is a Window with generalized active-target synchronisation (MPI-3 post / start /
+// complete / wait). Window itself is unchanged; reach these with a type assertion, w.(GroupWindow).
+// None of them is collective: only the ranks named in the groups take part. A group is a list of
+// distinct ranks; it may be empty or include this rank.
+//
+// Post opens an exposure epoch of this rank's window to origins and does not block. Start opens an
+// access epoch to targets and blocks until each has posted to this rank; after the watchdog_ms knob
+// it fails with a timeout, and no epoch is open. Complete closes the access epoch. Wait closes the
+// exposure epoch once every origin has completed; after watchdog_ms it fails with a timeout and the
+// epoch stays open. Test is Wait without waiting: true and closed, or false and still open. What an
+// origin put between Start and Complete is visible to the target once Wait returns. A rank with an
+// epoch open on a window must not Fence or Free it: that call fails on every rank.
+type GroupWindow interface {
+	Window
+	Post(origins []int) error
+	Start(targets []int) error
+	Complete() error
+	Wait() error
+	Test() (bool, error)
 }
 
 // Float32Loc, Float64Loc and Int64Loc are the elements of AllreduceLoc and ReduceLoc: a value and

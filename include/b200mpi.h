@@ -34,7 +34,8 @@ extern "C" {
                                then gather, scatter, gatherv, scatterv, allgatherv, alltoallv, scan, exscan,
                                reduce_scatterv, allreduce_loc, reduce_loc, win_create, win_free, win_fence,
                                put, get, accumulate, win_lock, win_unlock, get_accumulate, fetch_and_op,
-                               compare_and_swap (all additive) */
+                               compare_and_swap, win_post, win_start, win_complete, win_wait, win_test
+                               (all additive) */
 #define B200MPI_MAX_RANKS 8 /* "the 8 GPUs of one box" */
 
 typedef enum {
@@ -299,6 +300,43 @@ int b200mpi_fetch_and_op(const void* origin, void* result, int dtype, int op,
  * pointers to one element each, one kernel launch. */
 int b200mpi_compare_and_swap(const void* origin, const void* compare, void* result, int dtype,
                              int target, size_t target_disp, int win);
+
+/* ---- one-sided communication, generalized active target (MPI-3 post / start / complete / wait) --- */
+/* A group is `count` distinct ranks in [0, size()); it may include this rank, and count == 0 is legal
+ * (ranks may be NULL then).
+ * None of these calls is collective or takes a barrier epoch.  Each runs on the caller's collective thread.
+ *
+ * win_start blocks until every target in its group has posted an exposure epoch that includes this
+ * rank; then Put, Get and Accumulate to those targets are safe with no further waiting.  If a target
+ * has not posted within the watchdog_ms knob: B200MPI_ERR_TIMEOUT, and no access epoch is open; the
+ * posts that did arrive are not consumed, so a later win_start still sees them.  win_wait blocks until
+ * every origin of the post's group has called win_complete for this epoch; if that does not happen
+ * within watchdog_ms: B200MPI_ERR_TIMEOUT, and the exposure epoch stays open, so win_wait or win_test
+ * may be called again.  win_test checks once and never waits.  An empty group opens and closes its
+ * epoch without launching anything.
+ * Ordering: every Put and Accumulate an origin issued between its win_start and its win_complete is
+ * visible to the target, its own later kernels and copies included, once its win_wait returns (or
+ * win_test sets *flag = 1).  A Get issued after win_start reads what the target's window held when
+ * it called win_post.  The target's own writes to its window must be complete before win_post, and it
+ * must not change the window locally between win_post and win_wait, as MPI requires.  Put, Get and
+ * Accumulate are unchanged: they work inside or outside any epoch and do not check membership.
+ * Errors (B200MPI_ERR_ARG, nothing launched): an unknown or freed window; a group with a NULL pointer
+ * and count > 0, a negative count, count > size(), a rank out of range or a rank twice; win_post while
+ * this rank's exposure epoch on the window is open; win_start while its access epoch is open;
+ * win_complete with no access epoch open; win_wait or win_test with no exposure epoch open, or
+ * win_test with a NULL flag.
+ * Fences and locks: win_fence or win_free by a rank with an access or exposure epoch open on that
+ * window returns B200MPI_ERR_ARG there and B200MPI_ERR_PEER on every other rank (in a world of one:
+ * B200MPI_ERR_ARG, nothing launched), as under a held lock; the window stays live and the epoch open.
+ * Locks and these epochs on one window are independent: both may be used, in turn or at once.
+ * Erroneous programs: a target that posts to an origin which never starts on it (erroneous in MPI
+ * too) only makes that target's win_wait time out; its exposure epoch stays open, so that rank's
+ * win_fence and win_free of the window keep failing, until the origin starts and completes. */
+int b200mpi_win_post(const int* origins, int count, int win);   /* open an exposure epoch to `origins`; does not block */
+int b200mpi_win_start(const int* targets, int count, int win);  /* open an access epoch; blocks until every target has posted to this rank */
+int b200mpi_win_complete(int win);                              /* close the access epoch: tells each target this rank is done */
+int b200mpi_win_wait(int win);                                  /* close the exposure epoch: blocks until every origin has completed */
+int b200mpi_win_test(int win, int* flag);                       /* win_wait without blocking: *flag = 1 and the epoch closed, or 0 and still open */
 
 /* Enqueue-only forms on the library stream (DEVICE memkind only). */
 int b200mpi_bcast_async(void* buf, size_t count, int dtype, int root);

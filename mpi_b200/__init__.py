@@ -5,7 +5,8 @@ Init, Finalize, Rank, Size, Send, Receive (+ Recv, Bcast, Allreduce, Allgather, 
 ReduceScatter, Reduce, Alltoall, Gather, Scatter, Gatherv, Scatterv, Allgatherv, Alltoallv,
 Scan, Exscan, ReduceScatterv, AllreduceLoc, ReduceLoc (MAXLOC / MINLOC over the LOC_F32, LOC_F64
 and LOC_I64 pair dtypes), WinCreate (one-sided Put, Get and Accumulate through a Win, and the
-passive-target Lock, Unlock, GetAccumulate, FetchAndOp and CompareAndSwap), Isend/Wait).
+passive-target Lock, Unlock, GetAccumulate, FetchAndOp and CompareAndSwap, and the generalized
+active-target Post, Start, Complete, Wait and Test), Isend/Wait).
 The shared library (mpi_b200/lib/libb200mpi.so, built by mpi_b200/csrc/Makefile) is loaded on
 first use; nothing here computes or moves payload bytes in Python.
 """

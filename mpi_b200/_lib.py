@@ -71,6 +71,11 @@ SYMBOLS = {
     "b200mpi_get_accumulate": (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_size_t, _c.c_int, _c.c_int, _c.c_int, _c.c_size_t, _c.c_int, _c.c_int]),
     "b200mpi_fetch_and_op": (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_int, _c.c_int, _c.c_int, _c.c_size_t, _c.c_int]),
     "b200mpi_compare_and_swap": (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_int, _c.c_int, _c.c_size_t, _c.c_int]),
+    "b200mpi_win_post": (_c.c_int, [_c.c_void_p, _c.c_int, _c.c_int]),
+    "b200mpi_win_start": (_c.c_int, [_c.c_void_p, _c.c_int, _c.c_int]),
+    "b200mpi_win_complete": (_c.c_int, [_c.c_int]),
+    "b200mpi_win_wait": (_c.c_int, [_c.c_int]),
+    "b200mpi_win_test": (_c.c_int, [_c.c_int, _c.c_void_p]),
     "b200mpi_reduce_scatter_async": (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_size_t, _c.c_int, _c.c_int]),
     "b200mpi_numa_node": (_c.c_int, []),
     "b200mpi_barrier": (_c.c_int, []),

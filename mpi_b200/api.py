@@ -14,6 +14,7 @@ Same names, same argument meaning, same blocking behaviour:
     AllreduceLoc(send, recv, op)  ReduceLoc(send, recv, op, root)   (MAXLOC / MINLOC, new)
     WinCreate(local) -> Win: Put, Get, Accumulate, Fence, Free      (one-sided, fence-synchronised, new)
         + Lock, Unlock, GetAccumulate, FetchAndOp, CompareAndSwap   (passive target, new)
+        + Post, Start, Complete, Wait, Test                         (generalized active target, new)
     Isend(data, destination, tag) + Wait(destination, tag)     (the Send/Wait design commented out
                                                                 in the reference, mpi.go:132-152)
 
@@ -577,7 +578,15 @@ class Win:
     window without the other ranks taking part; every call has completed when it returns, so what a
     rank did under the lock is visible to the next holder.  GetAccumulate, FetchAndOp and
     CompareAndSwap return the target's previous values, one atomic per element.  A rank holding a lock
-    on this window must not Fence or Free it (MpiError, and the other ranks' call fails too)."""
+    on this window must not Fence or Free it (MpiError, and the other ranks' call fails too).
+
+    Generalized active target: a target calls Post(origins) to expose its window to a group of ranks
+    and Wait() (or Test()) to close that epoch; an origin calls Start(targets), which blocks until each
+    target has posted to it, and Complete() once its Put, Get and Accumulate calls are done.  Only the
+    ranks in the groups take part.  What the origins put between Start and Complete is visible to the
+    target once its Wait returns.  A group is an iterable of distinct ranks (Python or numpy ints),
+    possibly empty or containing this rank.  A rank with an epoch open on this window must not Fence
+    or Free it, as under a lock."""
 
     def __init__(self, wid):
         self.id = wid
@@ -672,6 +681,48 @@ class Win:
         res = np.zeros(1, dtype=np.int64)
         _check(L.load().b200mpi_compare_and_swap(v.ctypes.data, c.ctypes.data, res.ctypes.data, L.I64, int(target), int(disp), self.id))
         return res[0]
+
+    @staticmethod
+    def _group(ranks, what):
+        """A C int array of the ranks of an iterable of Python or numpy ints (range and duplicates are
+        the library's to check) and its length."""
+        try:
+            items = list(ranks)
+        except TypeError:
+            raise TypeError("mpi: %s takes an iterable of ranks, not %s" % (what, type(ranks).__name__)) from None
+        for r in items:
+            if isinstance(r, (bool, np.bool_)) or not isinstance(r, (int, np.integer)):
+                raise TypeError("mpi: %s takes ranks as ints, not %s" % (what, type(r).__name__))
+        arr = (ctypes.c_int * max(len(items), 1))()
+        for i, r in enumerate(items):
+            arr[i] = int(r) if -2**31 <= int(r) < 2**31 else -1  # -1: out of range, which the library refuses
+        return arr, len(items)
+
+    def Post(self, origins):
+        """Opens an exposure epoch of this window to the ranks in `origins`; does not block."""
+        arr, n = self._group(origins, "Post")
+        _check(L.load().b200mpi_win_post(arr, n, self.id))
+
+    def Start(self, targets):
+        """Opens an access epoch to the ranks in `targets`: blocks until each has posted to this rank
+        (MpiError ERR_TIMEOUT, and no epoch open, if one has not within the watchdog_ms knob)."""
+        arr, n = self._group(targets, "Start")
+        _check(L.load().b200mpi_win_start(arr, n, self.id))
+
+    def Complete(self):
+        """Closes the access epoch: tells each target of Start that this rank is done."""
+        _check(L.load().b200mpi_win_complete(self.id))
+
+    def Wait(self):
+        """Closes the exposure epoch once every origin of Post has called Complete (MpiError
+        ERR_TIMEOUT, the epoch still open, if they have not within the watchdog_ms knob)."""
+        _check(L.load().b200mpi_win_wait(self.id))
+
+    def Test(self):
+        """Wait without waiting: True and the exposure epoch closed, or False and still open."""
+        flag = ctypes.c_int(0)
+        _check(L.load().b200mpi_win_test(self.id, ctypes.byref(flag)))
+        return bool(flag.value)
 
     def Fence(self):
         _check(L.load().b200mpi_win_fence(self.id))

@@ -17,7 +17,8 @@
 //        Gather, Scatter, Gatherv, Scatterv, Allgatherv, Alltoallv, Scan, Exscan, ReduceScatterv,
 //        AllreduceLoc, ReduceLoc (MAXLOC / MINLOC over mpi::ValLoc<V> pairs),
 //        WinCreate -> mpi::Window with Put, Get, Accumulate, Fence, Free (one-sided, fence-synchronised)
-//        and Lock, Unlock, GetAccumulate, FetchAndOp, CompareAndSwap (passive target);
+//        and Lock, Unlock, GetAccumulate, FetchAndOp, CompareAndSwap (passive target)
+//        and Post, Start, Complete, Wait, Test (generalized active target);
 //        mpi::DeviceSlice<T> for heap-resident buffers
 // `data` may be std::vector<double|float|int64_t|uint8_t>, std::string (sent as bytes, the
 // "anything else is gob-encoded" path), or DeviceSlice<T>.
@@ -219,6 +220,12 @@ struct Interface {
   virtual Error GetAccumulate(Buffer, Buffer, Op, int, size_t, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no GetAccumulate"; return e; }
   virtual Error FetchAndOp(const void*, void*, int, Op, int, size_t, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no FetchAndOp"; return e; }
   virtual Error CompareAndSwap(const void*, const void*, void*, int, int, size_t, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no CompareAndSwap"; return e; }
+  // generalized active target: a group is (ranks, count); WinTest sets *flag to 1 or 0
+  virtual Error WinPost(const int*, int, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no WinPost"; return e; }
+  virtual Error WinStart(const int*, int, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no WinStart"; return e; }
+  virtual Error WinComplete(int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no WinComplete"; return e; }
+  virtual Error WinWait(int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no WinWait"; return e; }
+  virtual Error WinTest(int, int*) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no WinTest"; return e; }
   // the Send/Wait pair the reference sketches and comments out (mpi.go:132-152)
   virtual Error Isend(Buffer, int, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Isend"; return e; }
   virtual Error Wait(int, int) { Error e; e.code = B200MPI_ERR_UNSUPPORTED; e.msg = "registered implementation has no Wait"; return e; }
@@ -283,6 +290,11 @@ struct Cuda : Interface {
   Error CompareAndSwap(const void* o, const void* c, void* r, int dtype, int target, size_t disp, int win) override {
     return make_error(b200mpi_compare_and_swap(o, c, r, dtype, target, disp, win));
   }
+  Error WinPost(const int* origins, int count, int win) override { return make_error(b200mpi_win_post(origins, count, win)); }
+  Error WinStart(const int* targets, int count, int win) override { return make_error(b200mpi_win_start(targets, count, win)); }
+  Error WinComplete(int win) override { return make_error(b200mpi_win_complete(win)); }
+  Error WinWait(int win) override { return make_error(b200mpi_win_wait(win)); }
+  Error WinTest(int win, int* flag) override { return make_error(b200mpi_win_test(win, flag)); }
   Error Isend(Buffer d, int destination, int tag) override { return make_error(b200mpi_isend(d.ptr, d.count, d.dtype, destination, tag, d.memkind)); }
   Error Wait(int destination, int tag) override { return make_error(b200mpi_wait(destination, tag)); }
 };
@@ -499,7 +511,11 @@ template <typename V> inline Error ReduceLoc(const DeviceSlice<ValLoc<V>>& send,
 // Passive target: Lock / Unlock one target's window without the other ranks; GetAccumulate (the
 // result has the origin's type, length and storage, and may be the origin; NO_OP takes nullptr as
 // origin), FetchAndOp and CompareAndSwap (int64_t) return the target's previous values atomically.
-// A rank must not Fence or Free a window it holds a lock on.
+// Generalized active target: a target exposes its window to a group with Post and closes the epoch
+// with Wait (or Test, which never blocks); an origin opens an access epoch with Start, which blocks
+// until every target has posted to it, and closes it with Complete.  Only the ranks in the groups
+// take part; what an origin put between Start and Complete is visible to the target once its Wait
+// returns.  A rank must not Fence or Free a window it holds a lock or has an epoch open on.
 class Window {
  public:
   int id = -1;
@@ -530,6 +546,16 @@ class Window {
   template <typename T> Error Get(std::vector<T>* origin, int target, size_t disp) { return mpier()->Get(lower(*origin), target, disp, id); }
   template <typename T> Error Get(DeviceSlice<T>* origin, int target, size_t disp) { return mpier()->Get(lower(*origin), target, disp, id); }
   template <typename D> Error Accumulate(const D& origin, int target, size_t disp, Op op = SUM) { return mpier()->Accumulate(lower(origin), op, target, disp, id); }
+  Error Post(const std::vector<int>& origins) { return mpier()->WinPost(origins.data(), (int)origins.size(), id); }
+  Error Start(const std::vector<int>& targets) { return mpier()->WinStart(targets.data(), (int)targets.size(), id); }
+  Error Complete() { return mpier()->WinComplete(id); }
+  Error Wait() { return mpier()->WinWait(id); }
+  Error Test(bool* flag) { // *flag: the exposure epoch has ended (and is closed)
+    int f = 0;
+    Error e = mpier()->WinTest(id, &f);
+    if (!e) *flag = f != 0;
+    return e;
+  }
   Error Fence() { return mpier()->WinFence(id); }
   Error Free() { return mpier()->WinFree(id); }
 };

@@ -169,11 +169,15 @@ struct Ctx {
     uint64_t off[B200MPI_MAX_RANKS], bytes[B200MPI_MAX_RANKS];
     uint32_t lock_cell;                    // its lock word in every rank's control region (kWinLockOff)
     uint8_t held[B200MPI_MAX_RANKS];       // the lock this rank holds on each target's window: 0 none, or a b200mpi_lock_type
+    bool exposed, accessing;               // an exposure (win_post) / access (win_start) epoch of this rank is open
+    uint8_t expose_group, access_group;    // the members of the open epochs, as rank masks
+    uint16_t exposures[B200MPI_MAX_RANKS]; // exposure epochs this rank opened to each origin, mod 2^16
+    uint16_t accesses[B200MPI_MAX_RANKS];  // access epochs this rank started on each target, mod 2^16
   };
   std::vector<Win> wins;
   std::vector<bool> lock_cell_used;        // kWinLockCells entries, one per lock word; a freed window's cell is reused
   // Host-mapped pinned words (allocated on first use): [0] the value fetch_and_op and compare_and_swap
-  // fetch, [1] win_lock_try_kernel's verdict.
+  // fetch, [1] win_lock_try_kernel's verdict, [2] pscw_poll_kernel's arrivals (one byte per thread).
   uint64_t* rma_host = nullptr;
   uint64_t* rma_dev = nullptr;
 };
@@ -1577,12 +1581,12 @@ static int do_win_create(void* base, size_t bytes, int* win) {
   else if ((base || bytes) && (!base || bytes > g->heap.size || !g->heap.contains(base, bytes, off)))
     bad = "window memory must lie in this rank's b200mpi_alloc heap (or be 0 bytes at NULL)";
   // The lowest free lock cell: create and free are collective and run in the same order on every rank,
-  // so every rank picks the same one.  This rank zeroes its own word before the exchange, so no peer
-  // can lock it before it is clear.
+  // so every rank picks the same one.  This rank zeroes its own cell (the lock word and the PSCW
+  // counters) before the exchange, so no peer can lock it or signal into it before it is clear.
   g->lock_cell_used.resize(kWinLockCells);
   const uint64_t cell = std::find(g->lock_cell_used.begin(), g->lock_cell_used.end(), false) - g->lock_cell_used.begin();
   if (!bad && cell < kWinLockCells) {
-    CUDA_OK(cudaMemsetAsync((char*)g->heap.base[g->ctrl.rank] + kWinLockOff + cell * kWinLockStride, 0, sizeof(uint64_t), g->stream));
+    CUDA_OK(cudaMemsetAsync((char*)g->heap.base[g->ctrl.rank] + kWinLockOff + cell * kWinLockStride, 0, kWinLockStride, g->stream));
     CUDA_OK(cudaStreamSynchronize(g->stream));
   }
   struct { uint64_t id, off, bytes, bad, cell; } mine = {g->wins.size(), off, bytes, bad ? 1u : 0u, cell}, all[B200MPI_MAX_RANKS];
@@ -1606,17 +1610,23 @@ static int do_win_create(void* base, size_t bytes, int* win) {
 
 // Collective: the barrier kernel under signature 15 carrying the window id, so a fence on another
 // window or a Barrier ends as B200MPI_ERR_PEER on every rank.  A world of one synchronises the stream.
-// free: the window is dropped once the fence has succeeded.  A rank that holds a lock on the window
-// enters under a signature with the "locked" mark (extra = 1): the mismatch ends the call on every
-// rank, as B200MPI_ERR_ARG here and B200MPI_ERR_PEER on the others, and the window and lock stay.
+// free: the window is dropped once the fence has succeeded.  A rank that holds a lock on the window,
+// or has an access or exposure epoch open on it, enters under a signature with the "locked" mark
+// (extra = 1): the mismatch ends the call on every rank, as B200MPI_ERR_ARG here and
+// B200MPI_ERR_PEER on the others, and the window, the lock and the epochs stay.
 static int do_win_fence(int win, bool free) {
   const char* what = free ? "win_free" : "win_fence";
   int rc = need_data_plane();
   if (rc) return rc;
   Ctx::Win* w = find_win(win);
   if (!w) return unknown_win(what);
-  const bool locked = std::any_of(w->held, w->held + B200MPI_MAX_RANKS, [](uint8_t h) { return h != 0; });
-  const std::string held = std::string(what) + ": this rank holds a lock on the window (unlock it first)";
+  const bool holds = std::any_of(w->held, w->held + B200MPI_MAX_RANKS, [](uint8_t h) { return h != 0; });
+  const bool epoch = w->exposed || w->accessing;
+  const bool locked = holds || epoch;
+  const std::string held = std::string(what) + ": this rank " +
+                           (holds && epoch ? "holds a lock on the window and has an access or exposure epoch open on it (unlock it, and complete or wait the epoch, first)"
+                            : holds        ? "holds a lock on the window (unlock it first)"
+                                           : "has an access or exposure epoch open on the window (complete or wait it first)");
   if (locked && g->ctrl.n == 1) return fail(B200MPI_ERR_ARG, held);
   if (g->ctrl.n > 1 && (rc = launch_coll(barrier_kernel, "barrier_kernel", make_sig(15, 0, locked ? 1 : 0, 0, (size_t)win), 1, 32, 0, g->stream))) return rc;
   rc = finish(false);
@@ -1877,6 +1887,157 @@ static int do_compare_and_swap(const void* origin, const void* compare, void* re
   cas_kernel<<<1, 1, 0, g->stream>>>((unsigned long long*)remote, c, v, (unsigned long long*)g->rma_dev);
   if ((rc = launch_check("cas_kernel")) || (rc = finish(false))) return rc;
   memcpy(result, (const void*)g->rma_host, 8);
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Generalized active target: post / start / complete / wait / test.  Not collectives, no epoch, and
+// only the ranks named in a group take part.  Each pair of ranks counts its epochs on the window in
+// two 16-bit words of the window's cell (kPscwPostedOff, kPscwCompletedOff in kernels.cuh): post and
+// complete store the new count into the peer's cell (pscw_signal_kernel), start and wait poll this
+// rank's own cell for the count they expect (pscw_poll_kernel, relaunched for the members still
+// missing until all have arrived or watchdog_ms has passed).  Every call ends in a stream
+// synchronisation, which is the ordering argument of win_unlock (DESIGN §3).
+// ---------------------------------------------------------------------------------------------
+static uint16_t* pscw_word(const Ctx::Win* w, int owner, size_t off, int peer) {
+  return (uint16_t*)((char*)g->heap.base[owner] + kWinLockOff + (size_t)w->lock_cell * kWinLockStride + off) + peer;
+}
+
+// `count` distinct ranks in [0, size()) as a mask; nullptr when well formed, else what is wrong.
+static const char* pscw_group(const int* ranks, int count, uint8_t& mask) {
+  mask = 0;
+  if (count < 0) return "negative group size";
+  if (count > g->ctrl.n) return "group larger than the world";
+  if (count > 0 && !ranks) return "NULL group with count > 0";
+  for (int i = 0; i < count; ++i) {
+    if (ranks[i] < 0 || ranks[i] >= g->ctrl.n) return "rank in the group out of range";
+    if (mask >> ranks[i] & 1) return "rank repeated in the group";
+    mask |= (uint8_t)(1u << ranks[i]);
+  }
+  return nullptr;
+}
+
+// Stores count[r] into the word `off` of every member r's cell at index this rank: one launch, none
+// for an empty group.
+static int pscw_signal(const Ctx::Win* w, uint8_t mask, size_t off, const uint16_t* count) {
+  PscwGroup grp{};
+  int m = 0;
+  for (int r = 0; r < g->ctrl.n; ++r)
+    if (mask >> r & 1) {
+      grp.word[m] = pscw_word(w, r, off, g->ctrl.rank);
+      grp.count[m++] = count[r];
+    }
+  if (m == 0) return 0;
+  pscw_signal_kernel<<<1, m, 0, g->stream>>>(grp);
+  const int rc = launch_check("pscw_signal_kernel");
+  return rc ? rc : finish(false);
+}
+
+// Polls the words `off` of this rank's cell at the members of `mask` until each holds want[r]: one
+// launch per pass, the next pass for the members still missing, a single pass of one attempt for
+// `once` (win_test).  `all`: every member arrived.  An empty group launches nothing.
+static int pscw_poll(const Ctx::Win* w, uint8_t mask, size_t off, const uint16_t* want, bool once, bool& all) {
+  int rc = need_rma_words();
+  if (rc) return rc;
+  volatile uint8_t* arrived = (volatile uint8_t*)(g->rma_host + 2);
+  Spinner sp(g->watchdog_ns);
+  uint8_t missing = mask;
+  while (missing) {
+    PscwGroup grp{};
+    int ranks[B200MPI_MAX_RANKS], m = 0;
+    for (int r = 0; r < g->ctrl.n; ++r)
+      if (missing >> r & 1) {
+        grp.word[m] = pscw_word(w, g->ctrl.rank, off, r);
+        grp.count[m] = want[r];
+        ranks[m++] = r;
+      }
+    for (int i = 0; i < m; ++i) arrived[i] = 2;
+    pscw_poll_kernel<<<1, m, 0, g->stream>>>(grp, once ? 1 : kPscwAttempts, (uint8_t*)(g->rma_dev + 2));
+    if ((rc = launch_check("pscw_poll_kernel")) || (rc = finish(false))) return rc;
+    for (int i = 0; i < m; ++i)
+      if (arrived[i] == 1) missing &= (uint8_t)~(1u << ranks[i]);
+    if (once || sp.expired()) break;
+  }
+  all = missing == 0;
+  return 0;
+}
+
+// The checks every PSCW call makes first, in this order: the data plane, the window, then (post and
+// start) the group.
+static int pscw_checks(const char* what, int win, Ctx::Win*& w, const int* ranks = nullptr, int count = 0, uint8_t* mask = nullptr) {
+  int rc = need_data_plane();
+  if (rc) return rc;
+  if (!(w = find_win(win))) return unknown_win(what);
+  if (mask)
+    if (const char* bad = pscw_group(ranks, count, *mask)) return fail(B200MPI_ERR_ARG, std::string(what) + ": " + bad);
+  return 0;
+}
+
+// Opens an exposure epoch to `origins`: their posted[this rank] words take the epoch's count.
+static int do_win_post(const int* origins, int count, int win) {
+  Ctx::Win* w = nullptr;
+  uint8_t mask = 0;
+  int rc = pscw_checks("win_post", win, w, origins, count, &mask);
+  if (rc) return rc;
+  if (w->exposed) return fail(B200MPI_ERR_ARG, "win_post: this rank's exposure epoch on the window is open already (win_wait closes it)");
+  uint16_t next[B200MPI_MAX_RANKS];
+  for (int r = 0; r < B200MPI_MAX_RANKS; ++r) next[r] = (uint16_t)(w->exposures[r] + 1);
+  if ((rc = pscw_signal(w, mask, kPscwPostedOff, next))) return rc;
+  for (int r = 0; r < g->ctrl.n; ++r)
+    if (mask >> r & 1) w->exposures[r] = next[r];
+  w->exposed = true;
+  w->expose_group = mask;
+  return 0;
+}
+
+// Opens an access epoch to `targets` once each has posted to this rank: posted[t] reaches the count
+// of this start.  On a timeout nothing changes, so a post that did arrive is seen by the next start.
+static int do_win_start(const int* targets, int count, int win) {
+  Ctx::Win* w = nullptr;
+  uint8_t mask = 0;
+  int rc = pscw_checks("win_start", win, w, targets, count, &mask);
+  if (rc) return rc;
+  if (w->accessing) return fail(B200MPI_ERR_ARG, "win_start: this rank's access epoch on the window is open already (win_complete closes it)");
+  uint16_t next[B200MPI_MAX_RANKS];
+  for (int r = 0; r < B200MPI_MAX_RANKS; ++r) next[r] = (uint16_t)(w->accesses[r] + 1);
+  bool all = false;
+  if ((rc = pscw_poll(w, mask, kPscwPostedOff, next, false, all))) return rc;
+  if (!all) return fail(B200MPI_ERR_TIMEOUT, "win_start: a target did not post to this rank within watchdog_ms; no access epoch is open");
+  for (int r = 0; r < g->ctrl.n; ++r)
+    if (mask >> r & 1) w->accesses[r] = next[r];
+  w->accessing = true;
+  w->access_group = mask;
+  return 0;
+}
+
+// Closes the access epoch: every target's completed[this rank] word takes the epoch's count.
+static int do_win_complete(int win) {
+  Ctx::Win* w = nullptr;
+  int rc = pscw_checks("win_complete", win, w);
+  if (rc) return rc;
+  if (!w->accessing) return fail(B200MPI_ERR_ARG, "win_complete: this rank has no access epoch open on the window");
+  if ((rc = pscw_signal(w, w->access_group, kPscwCompletedOff, w->accesses))) return rc;
+  w->accessing = false;
+  w->access_group = 0;
+  return 0;
+}
+
+// Closes the exposure epoch once every origin has completed: completed[o] reaches the count of the
+// post.  win_wait (flag == nullptr) waits up to watchdog_ms; win_test looks once.  Either way an epoch
+// that has not ended stays open.
+static int do_win_wait(int win, int* flag, bool test) {
+  const char* what = test ? "win_test" : "win_wait";
+  Ctx::Win* w = nullptr;
+  int rc = pscw_checks(what, win, w);
+  if (rc) return rc;
+  if (test && !flag) return fail(B200MPI_ERR_ARG, "win_test: NULL flag");
+  if (!w->exposed) return fail(B200MPI_ERR_ARG, std::string(what) + ": this rank has no exposure epoch open on the window");
+  bool all = false;
+  if ((rc = pscw_poll(w, w->expose_group, kPscwCompletedOff, w->exposures, test, all))) return rc;
+  if (test) *flag = all ? 1 : 0;
+  if (!all) return test ? 0 : fail(B200MPI_ERR_TIMEOUT, "win_wait: an origin did not complete within watchdog_ms; the exposure epoch stays open");
+  w->exposed = false;
+  w->expose_group = 0;
   return 0;
 }
 
@@ -2640,6 +2801,11 @@ int b200mpi_fetch_and_op(const void* origin, void* result, int dtype, int op, in
 int b200mpi_compare_and_swap(const void* origin, const void* compare, void* result, int dtype, int target, size_t target_disp, int win) {
   return do_compare_and_swap(origin, compare, result, dtype, target, target_disp, win);
 }
+int b200mpi_win_post(const int* origins, int count, int win) { return do_win_post(origins, count, win); }
+int b200mpi_win_start(const int* targets, int count, int win) { return do_win_start(targets, count, win); }
+int b200mpi_win_complete(int win) { return do_win_complete(win); }
+int b200mpi_win_wait(int win) { return do_win_wait(win, nullptr, false); }
+int b200mpi_win_test(int win, int* flag) { return do_win_wait(win, flag, true); }
 int b200mpi_gather(const void* send, void* recv, size_t count_per_rank, int dtype, int root, int memkind) { return do_gather(send, recv, count_per_rank, dtype, root, memkind, false); }
 int b200mpi_scatter(const void* send, void* recv, size_t count_per_rank, int dtype, int root, int memkind) { return do_gather(send, recv, count_per_rank, dtype, root, memkind, true); }
 int b200mpi_gatherv(const void* send, void* recv, const size_t* counts, int dtype, int root, int memkind) { return do_gatherv(send, recv, counts, dtype, root, false, memkind); }

@@ -8,7 +8,7 @@
 // The first kCtrlBytes of each heap are control words:
 //     Slot slots[kMaxBlocks][kMaxRanks]   cross-rank flag + per-call buffer descriptor
 //     u32  ring[kMaxBlocks]               ring step counters
-//     LL cells (kLLOff), window lock words (kWinLockOff)
+//     LL cells (kLLOff), window cells: lock word and PSCW counters (kWinLockOff)
 // A collective kernel is   sync_start -> body -> sync_end   where both syncs are per-CTA
 // barriers between the CTAs with the same blockIdx on every rank (flag writes with
 // st.release.sys into the peer's slot, ld.acquire.sys spins on the own slot).  sync_start also
@@ -2316,6 +2316,57 @@ __global__ void win_unlock_kernel(unsigned long long* word, int exclusive) {
   unsigned long long old;
   if (exclusive) asm volatile("atom.release.sys.global.and.b64 %0, [%1], %2;" : "=l"(old) : "l"(word), "l"(~kLockExclusive) : "memory");
   else asm volatile("atom.release.sys.global.add.u64 %0, [%1], %2;" : "=l"(old) : "l"(word), "l"(~0ull) : "memory");
+}
+
+// ---------------------------------------------------------------------------------------------
+// Generalized active target (b200mpi_win_post / _start / _complete / _wait / _test).  Two 16-bit
+// counters per pair of ranks and window, in the window's lock cell past the lock word:
+//   posted[t]    in origin o's cell, written only by target t: the exposure epochs t opened to o
+//   completed[o] in target t's cell, written only by origin o: the access epochs o closed on t
+// Each writer stores a count the host already knows, so no read-modify-write is needed.  A counter
+// never runs more than one ahead of its reader's expectation (DESIGN §3), so a poll tests for
+// equality with that count, modulo 2^16.
+// ---------------------------------------------------------------------------------------------
+constexpr size_t kPscwPostedOff = 8;     // u16 posted[kMaxRanks]
+constexpr size_t kPscwCompletedOff = 24; // u16 completed[kMaxRanks]
+static_assert(kPscwPostedOff >= sizeof(unsigned long long), "PSCW counters overlap the lock word");
+static_assert(kPscwCompletedOff >= kPscwPostedOff + kMaxRanks * sizeof(uint16_t), "posted and completed counters overlap");
+static_assert(kPscwCompletedOff + kMaxRanks * sizeof(uint16_t) <= kWinLockStride, "PSCW counters end past the window's cell");
+// Attempts one pscw_poll_kernel makes at each word, with the lock's __nanosleep backoff (about 0.25
+// ms in all), before it reports the members still missing and the host relaunches it.  A guess, not
+// a measurement, as kLockAttempts is: it bounds the kernel, and watchdog_ms bounds the wait.
+constexpr int kPscwAttempts = 256;
+
+// One entry per group member: the counter word (a peer's cell for a signal, this rank's own cell for
+// a poll) and the count to store or to wait for.
+struct PscwGroup {
+  uint16_t* word[kMaxRanks];
+  uint16_t count[kMaxRanks];
+};
+
+// Post and complete, one thread per member: st.release.sys of the new count.  The release orders this
+// rank's earlier window work before the peer's acquire: those kernels completed before this one
+// started, as for win_unlock_kernel.
+__global__ void pscw_signal_kernel(const __grid_constant__ PscwGroup grp) {
+  const int i = threadIdx.x;
+  asm volatile("st.release.sys.global.u16 [%0], %1;" ::"l"(grp.word[i]), "h"(grp.count[i]) : "memory");
+}
+
+// Start, wait and test, one thread per member: up to `attempts` ld.acquire.sys of its word, then
+// arrived[i] (host-mapped) = 1 if the word held its count, else 0.  Bounded, and it touches neither
+// the device watchdog nor the status word: a rank waiting for its peers is not a collective that
+// failed.
+__global__ void pscw_poll_kernel(const __grid_constant__ PscwGroup grp, int attempts, uint8_t* arrived) {
+  const int i = threadIdx.x;
+  unsigned ns = 32;
+  for (int a = 0; a < attempts; ++a) {
+    uint16_t v;
+    asm volatile("ld.acquire.sys.global.u16 %0, [%1];" : "=h"(v) : "l"(grp.word[i]) : "memory");
+    if (v == grp.count[i]) { *(volatile uint8_t*)(arrived + i) = 1; return; }
+    if (a + 1 < attempts) __nanosleep(ns);
+    if (ns < 1024) ns *= 2;
+  }
+  *(volatile uint8_t*)(arrived + i) = 0;
 }
 
 } // namespace b200

@@ -603,6 +603,66 @@ def main():
             for b in (wmem, org, res):
                 b.free()
 
+    if "pscw" in colls:
+        # One epoch of a ring neighbour exchange (medians of 200 epochs after 20, max over ranks): every
+        # rank Posts to and Starts on {left, right}, Puts S bytes into each, then Completes and Waits;
+        # beside it the same Puts closed by one win_fence.  S = 8 B and 1 MiB.
+        card = {}
+        try:  # a read-only query: the numbers belong next to the card and its power limit
+            q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", str(lib.b200mpi_device())],
+                               capture_output=True, text=True, timeout=30).stdout.strip().split(", ")
+            card = {"gpu": q[0], "power_limit": q[1]} if len(q) == 2 else {}
+        except (OSError, subprocess.SubprocessError):
+            pass
+        if n < 2 or L.get_param("shared_device"):
+            emit(dict({"coll": "pscw", "ok": True, "note": "fewer than two NVLink-connected GPUs (ranks %s): the PSCW and fence "
+                       "neighbour-exchange epochs not measured" % ("share one GPU" if n > 1 else "= 1")}, **card))
+        else:
+            left, right = (rank - 1) % n, (rank + 1) % n
+            nbrs = sorted({left, right})
+            for S in (8, 1 << 20):
+                e = S // 8
+                wmem = mpi.Alloc(2 * e, np.float64).copy_from_host(np.zeros(2 * e))
+                org = mpi.Alloc(e, np.float64).copy_from_host(np.full(e, rank + 1.0))
+                w = mpi.WinCreate(wmem)
+
+                def put_both():
+                    # slot 0 of the right neighbour holds its left's data, slot 1 of the left its right's
+                    for t, slot in ((right, 0), (left, 1)):
+                        if lib.b200mpi_put(org.ptr, e, L.F64, t, slot * e, w.id, L.DEVICE):
+                            raise RuntimeError(L.last_error())
+
+                def pscw_epoch():
+                    w.Post(nbrs)
+                    w.Start(nbrs)
+                    put_both()
+                    w.Complete()
+                    w.Wait()
+
+                def fence_epoch():
+                    put_both()
+                    w.Fence()
+
+                res = {}
+                for name, epoch in (("pscw", pscw_epoch), ("fence", fence_epoch)):
+                    mpi.Barrier()
+                    ts = []
+                    for i in range(220):
+                        t0 = time.perf_counter()
+                        epoch()
+                        ts.append(time.perf_counter() - t0)
+                    res[name] = maxr(sorted(ts[20:])[100])
+                    w.Fence()
+                    got = wmem.to_host()
+                    ok = bool(np.all(got[:e] == left + 1.0) and np.all(got[e:] == right + 1.0))
+                    res[name + "_ok"] = bool(maxr(0.0 if ok else 1.0) == 0.0)
+                emit(dict({"coll": "pscw", "bytes": S, "t_epoch_us_median": res["pscw"] * 1e6,
+                           "fence_t_epoch_us_median": res["fence"] * 1e6, "fence_over_pscw": res["fence"] / res["pscw"],
+                           "ok": res["pscw_ok"] and res["fence_ok"]}, **card))
+                w.Free()
+                wmem.free()
+                org.free()
+
     if "p2p" in colls and n > 1:
         # bounce (examples/bounce/bounce.go:85-138): even sends, odd returns; device-resident float64
         maxp = min(args.max_bytes, 256 << 20)
